@@ -77,7 +77,12 @@ typedef enum {
                         bit 1 = dropnan.  b200_agg_input: `mask` = validity (1 = value present, 0 = null row: the reference's
                         data mask), `order` = selection mask (uint8, 1 = the row takes part: set_selection_mask); both nullable */,
     B200_AGG_LIST /* AggList_<T>(grid, grids, threads, dropnan, dropnull) (src/agg_list.cpp:5-127): `moment` bit 0 = dropnan, bit 1 =
-                     dropnull; read with b200_agg_list_finish / b200_agg_list_read, not b200_agg_read */
+                     dropnull; read with b200_agg_list_finish / b200_agg_list_read, not b200_agg_read */,
+    B200_AGG_LIST_STRING /* AggList_string_int64(grid, grids, threads, dropnan, dropnull) (src/agg_list.cpp:122-222): `moment` bit 1 =
+                            dropnull, bit 0 (dropnan) is accepted and has no effect.  b200_agg_input: `data` = int64 offsets[nrows + 1],
+                            `order` = the bytes, indexed by those (absolute) offsets like b200_strset_update's, `mask` = validity (1 =
+                            string present, 0 = null, like NUNIQUE's; nullable).  No data mask: the reference never reads it.  Read
+                            with b200_agg_list_finish / b200_agg_list_string_bytes / b200_agg_list_string_read */
 } b200_agg_op;
 
 /* where the column pointers of a call live.  MIXED: every pointer is classified on its own (cudaPointerGetAttributes);
@@ -169,6 +174,12 @@ int b200_agg_merge(b200_agg *agg, b200_agg *const *others, int nothers);
  * offsets[cells + 1] and `total` values of the aggregator's dtype.  merge() is a no-op like the reference's (:46). */
 int b200_agg_list_finish(b200_agg *agg, int64_t *total_out);
 int b200_agg_list_read(b200_agg *agg, int64_t *offsets_out, void *values_out);
+/* AggList_string results (src/agg_list.cpp:160-194 get_result: list_from_arrays(offsets, StringList64)): per cell its strings in
+ * arrival order, a null where a null string arrived (unless dropnull).  After b200_agg_list_finish (which also gathers the strings):
+ * string_bytes = the elements' total byte count; string_read fills (each output nullable) list offsets int64[cells + 1], string
+ * offsets int64[total + 1], the bytes, and one validity byte per element (1 = string, 0 = null; a null is an empty string). */
+int b200_agg_list_string_bytes(b200_agg *agg, int64_t *nbytes_out);
+int b200_agg_list_string_read(b200_agg *agg, int64_t *list_offsets_out, int64_t *str_offsets_out, uint8_t *bytes_out, uint8_t *valid_out);
 /* load a full grid (result dtype, `cells` long) — TaskPartAggregation initial_values (vaex/cpu.py:654-658) */
 int b200_agg_write(b200_agg *agg, const void *values);
 

@@ -199,6 +199,86 @@ def main():
             report("SG", "df.groupby([k1,k2], combine=True).agg({v:[sum,count]}): 2 key sets + combined-code set, then fused probe pass", n, 24 + 24,
                    (t_keys + t_agg) * 1e3, groups=len(out["count"]), key_sets_ms=t_keys * 1e3, aggregate_ms=t_agg * 1e3)
             del k1, k2, v
+        elif cfg == "LS":
+            ls_string_list(args, ctx, stream, gen, report)
+
+
+def ls_string_list(args, ctx, stream, gen, report):
+    """LS: df.list(s, binby=g) over 1e8 device-resident strings of 1-32 bytes drawn from a 10^4-word vocabulary, 1e5 ordinal groups
+    (AggList_string_int64, csrc/list.cu).  The append pass (one bin() call), the finish on the device (sort + gather) and the D2H of
+    the arrow buffers are timed separately with CUDA events on the library's stream; the best of --reps rounds is reported."""
+    import numpy as np
+    import torch
+    from vaex_b200 import superagg
+    n, groups, vocab = 100_000_000, 100_000, 10_000
+    vlen = torch.randint(1, 33, (vocab,), device="cuda", generator=gen)
+    word = torch.randint(0, vocab, (n,), device="cuda", generator=gen)
+    lengths = vlen[word]
+    offsets = torch.zeros(n + 1, dtype=torch.int64, device="cuda")
+    torch.cumsum(lengths, 0, out=offsets[1:])
+    nbytes = int(offsets[-1])
+    data = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    step = 10_000_000
+    for r0 in range(0, n, step):  # byte p of a row's string = 'a' + (word * 7 + p) % 26: equal words give equal strings
+        r1 = min(r0 + step, n)
+        b0, b1 = int(offsets[r0]), int(offsets[r1])
+        row = torch.repeat_interleave(torch.arange(r0, r1, device="cuda"), lengths[r0:r1])
+        pos = torch.arange(b0, b1, device="cuda") - offsets[row]
+        data[b0:b1] = (97 + (word[row] * 7 + pos) % 26).to(torch.uint8)
+        del row, pos
+    keys = torch.randint(0, groups, (n,), device="cuda", dtype=torch.int32, generator=gen)
+    torch.cuda.synchronize()
+    b = superagg.BinnerOrdinal_int32(1, "g", groups, 0, False, False)
+    g = superagg.Grid([b])
+    a = superagg.AggList_string_int64(g, 1, 1)
+    b.set_data(0, keys)
+    a.set_buffers(0, offsets, data)
+    import ctypes as C
+    from vaex_b200 import _lib
+    L = _lib.lib()
+    cells = len(g)
+    lo, so, va = np.empty(cells + 1, np.int64), np.empty(n + 1, np.int64), np.empty(n, np.uint8)
+    by = np.empty(nbytes, np.uint8)
+    for arr in (lo, so, va, by):  # fault the host pages in once, outside the timed copies
+        arr.fill(0)
+    best = {}
+    for rep in range(args.reps + 1):  # round 0 warms up (pool and record arrays grow to size there)
+        a.reset(0)
+        e = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        e[0].record(stream)
+        g.bin(0, [a], n)
+        e[1].record(stream)
+        total, nb = C.c_int64(0), C.c_int64(0)
+        _lib.check(L.b200_agg_list_finish(a._h, C.byref(total)))  # sort + count + length scan + gather, on the same stream
+        _lib.check(L.b200_agg_list_string_bytes(a._h, C.byref(nb)))
+        e[2].record(stream)
+        _lib.check(L.b200_agg_list_string_read(a._h, lo.ctypes.data, so.ctypes.data, by.ctypes.data, va.ctypes.data))
+        e[3].record(stream)
+        ctx.sync()
+        torch.cuda.synchronize()
+        assert total.value == n and nb.value == nbytes
+        if rep:
+            for k, (i, j) in dict(append=(0, 1), finish=(1, 2), d2h=(2, 3)).items():
+                best[k] = min(best.get(k, float("inf")), e[i].elapsed_time(e[j]))
+    assert lo[-1] == n and so[-1] == nbytes and va.all()
+    best_append = best["append"]
+    mean = nbytes / n
+    radix_passes = 3  # keys < 2^17 (groups + 2 cells): three 8-bit passes
+    # algorithmic bytes per row.  append: key 4 + offsets 8 read, string read + written to the pool, key/payload/start 24 written.
+    # finish: per radix pass key + payload read and written (32), the count pass reads keys (8), lengths read payload + two starts
+    # and write the length (32), the int64 scan reads + writes it twice (32), the gather reads payload, start, two offsets and the
+    # string and writes the string and a validity byte (33 + 2 * mean); the D2H (into pageable numpy memory whose pages are already
+    # faulted in) moves the string offsets, bytes and validity (9 + mean) over PCIe, so its rate is not an HBM figure
+    append_bpr = 4 + 8 + 2 * mean + 24
+    finish_bpr = 32 * radix_passes + 8 + 32 + 32 + 33 + 2 * mean
+    d2h_bpr = 9 + mean
+    report("LS/append", "AggList_string_int64 append: one bin() call over 1e8 device strings of 1-32 B, 1e5 ordinal groups", n, append_bpr, best_append,
+           string_bytes=nbytes, mean_string_bytes=mean)
+    report("LS/finish", "AggList_string_int64 finish on the device: radix sort by cell + per-cell count + int64 length scan + byte gather", n,
+           finish_bpr, best["finish"], string_bytes=nbytes, radix_passes=radix_passes)
+    report("LS/d2h", "AggList_string_int64 read: D2H of the arrow buffers into pageable numpy arrays", n, d2h_bpr, best["d2h"], string_bytes=nbytes)
+    report("LS/finish+d2h", "AggList_string_int64 result: finish + D2H", n, finish_bpr + d2h_bpr, best["finish"] + best["d2h"], string_bytes=nbytes)
+    del offsets, data, keys, word, lengths
 
 
 if __name__ == "__main__":

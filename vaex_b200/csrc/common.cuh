@@ -142,6 +142,16 @@ struct b200_agg {
     unsigned *list_counts = nullptr;       // after finish: exclusive offsets per cell (+ the total)
     uint64_t list_n = 0, list_cap = 0, list_total = 0;
     bool list_sorted = false;
+    // LIST_STRING (list.cu): the same records (key = cell, payload = record index | null << 63); every call appends its byte range
+    // to `lstr_pool` and list_starts[i] is where record i's string starts there (list_cap + 1 entries: the last one closes the pool)
+    unsigned long long *list_starts = nullptr;
+    char *lstr_pool = nullptr;
+    uint64_t lstr_pool_n = 0, lstr_pool_cap = 0;
+    // after finish: int64 string offsets[list_total + 1], the gathered bytes, one validity byte per element
+    long long *lstr_off = nullptr;
+    char *lstr_bytes = nullptr;
+    uint8_t *lstr_valid = nullptr;
+    uint64_t lstr_nbytes = 0;
 };
 
 namespace b200 {

@@ -18,6 +18,7 @@
 #include "device_utils.cuh"
 #include "radix.cuh"
 #include "scan.cuh"
+#include "strings.cuh"
 
 namespace b200 {
 struct StrLog {
@@ -1322,45 +1323,6 @@ __global__ void k_str_gather(const unsigned long long *str_off, const unsigned *
     }
 }
 
-// string columns staged for one call: offsets (device), bytes (device, starting at offsets[0]), masks
-struct StrInput {
-    const long long *offsets = nullptr;
-    const unsigned char *bytes = nullptr;
-    const uint8_t *masks = nullptr;
-    long long base = 0, nbytes = 0;
-};
-
-int stage_strings(b200_ctx *ctx, Slot *sl, Stager &stg, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, int memspace, StrInput *in) {
-    long long first = 0, last = 0;
-    if (nrows) {
-        if (memspace == B200_MEM_DEVICE) {
-            B200_CUDA(cudaMemcpyAsync(&first, offsets, 8, cudaMemcpyDeviceToHost, sl->stream));
-            B200_CUDA(cudaMemcpyAsync(&last, offsets + nrows, 8, cudaMemcpyDeviceToHost, sl->stream));
-            B200_CUDA(cudaStreamSynchronize(sl->stream));
-        } else {
-            first = offsets[0], last = offsets[nrows];
-        }
-    }
-    in->base = first;
-    in->nbytes = last - first;
-    stg.plan(offsets, (size_t)(nrows + 1) * 8);
-    if (in->nbytes)
-        stg.plan(bytes + (memspace == B200_MEM_DEVICE ? 0 : first), (size_t)in->nbytes);
-    if (masks)
-        stg.plan(masks, (size_t)nrows);
-    B200_CHECK(stg.commit());
-    in->offsets = static_cast<const long long *>(stg.dev(offsets));
-    if (memspace == B200_MEM_DEVICE) {
-        in->bytes = bytes; // device: index with the absolute offsets
-        in->base = 0;
-    } else {
-        in->bytes = in->nbytes ? static_cast<const unsigned char *>(stg.dev(bytes + first)) : bytes;
-    }
-    in->masks = masks ? static_cast<const uint8_t *>(stg.dev(masks)) : nullptr;
-    (void)ctx;
-    return B200_OK;
-}
-
 int str_finalize(b200_set *s) { // caller holds s->mu
     const bool was_dirty = s->dirty;
     B200_CHECK(set_finalize(s));
@@ -1437,7 +1399,7 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
     cudaStream_t st = sl->stream;
     Stager stg{s->ctx, sl, memspace};
     StrInput in;
-    B200_CHECK(stage_strings(s->ctx, sl, stg, offsets, bytes, masks, nrows, memspace, &in));
+    B200_CHECK(stage_strings(sl, stg, offsets, bytes, masks, nrows, memspace, &in));
     // room for the worst case of this call: every row a new key
     {
         uint64_t want = s->cap;
@@ -1526,7 +1488,7 @@ int b200_strset_map_ordinal(b200_set *s, int slot, const int64_t *offsets, const
     B200_CHECK(str_finalize(s));
     Stager stg{s->ctx, sl, memspace};
     StrInput in;
-    B200_CHECK(stage_strings(s->ctx, sl, stg, offsets, bytes, masks, nrows, memspace, &in));
+    B200_CHECK(stage_strings(sl, stg, offsets, bytes, masks, nrows, memspace, &in));
     long long *d_out = out_is_device ? reinterpret_cast<long long *>(out) : nullptr;
     if (!out_is_device)
         B200_CUDA(cudaMalloc(&d_out, sizeof(long long) * nrows));
