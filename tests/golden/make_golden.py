@@ -22,44 +22,49 @@ from oracle import oracle as O  # noqa: E402
 from oracle import ref_driver as R  # noqa: E402
 
 
+def add_case(out, name, binners, aggs, n):
+    """run the compiled reference on one (binners, aggs) problem; store inputs and outputs as `name/<field>` arrays in `out`"""
+    res = R.binby(binners, aggs, n)
+    c = {"n": n, "nb": len(binners), "na": len(aggs)}
+    for i, b in enumerate(binners):
+        c[f"b{i}_kind"] = b["kind"]
+        c[f"b{i}_data"] = b["data"]
+        c[f"b{i}_dtype"] = b["data"].dtype.str  # npz drops byte order
+        if b["mask"] is not None:
+            c[f"b{i}_mask"] = b["mask"]
+        for k in ("vmin", "vmax", "bins", "count", "min_value", "allow_other", "invert"):
+            if k in b:
+                c[f"b{i}_{k}"] = b[k]
+    for k, (a, r) in enumerate(zip(aggs, res)):
+        c[f"a{k}_op"] = a["op"]
+        if a["data"] is not None:
+            c[f"a{k}_data"] = a["data"]
+            c[f"a{k}_dtype"] = a["data"].dtype.str
+        if a["mask"] is not None:
+            c[f"a{k}_mask"] = a["mask"]
+        if a.get("moment") is not None:
+            c[f"a{k}_moment"] = a["moment"]
+        if a.get("order") is not None:
+            c[f"a{k}_order"] = a["order"]
+        if a.get("selection") is not None:
+            c[f"a{k}_selection"] = a["selection"]
+        if a["op"] == "nunique":
+            c[f"a{k}_drop"] = np.array([a["dropmissing"], a["dropnan"]])
+        if np.ma.isMaskedArray(r):
+            c[f"a{k}_result"] = np.asarray(r.data)
+            c[f"a{k}_result_mask"] = np.ma.getmaskarray(r)
+        else:
+            c[f"a{k}_result"] = np.asarray(r)
+    for k, v in c.items():
+        out[f"{name}/{k}"] = np.asarray(v)
+
+
 def cases():
     rng = np.random.default_rng(20260922)
     out = {}
 
     def add(name, binners, aggs, n):
-        res = R.binby(binners, aggs, n)
-        c = {"n": n, "nb": len(binners), "na": len(aggs)}
-        for i, b in enumerate(binners):
-            c[f"b{i}_kind"] = b["kind"]
-            c[f"b{i}_data"] = b["data"]
-            c[f"b{i}_dtype"] = b["data"].dtype.str  # npz drops byte order
-            if b["mask"] is not None:
-                c[f"b{i}_mask"] = b["mask"]
-            for k in ("vmin", "vmax", "bins", "count", "min_value", "allow_other", "invert"):
-                if k in b:
-                    c[f"b{i}_{k}"] = b[k]
-        for k, (a, r) in enumerate(zip(aggs, res)):
-            c[f"a{k}_op"] = a["op"]
-            if a["data"] is not None:
-                c[f"a{k}_data"] = a["data"]
-                c[f"a{k}_dtype"] = a["data"].dtype.str
-            if a["mask"] is not None:
-                c[f"a{k}_mask"] = a["mask"]
-            if a.get("moment") is not None:
-                c[f"a{k}_moment"] = a["moment"]
-            if a.get("order") is not None:
-                c[f"a{k}_order"] = a["order"]
-            if a.get("selection") is not None:
-                c[f"a{k}_selection"] = a["selection"]
-            if a["op"] == "nunique":
-                c[f"a{k}_drop"] = np.array([a["dropmissing"], a["dropnan"]])
-            if np.ma.isMaskedArray(r):
-                c[f"a{k}_result"] = np.asarray(r.data)
-                c[f"a{k}_result_mask"] = np.ma.getmaskarray(r)
-            else:
-                c[f"a{k}_result"] = np.asarray(r)
-        for k, v in c.items():
-            out[f"{name}/{k}"] = np.asarray(v)
+        add_case(out, name, binners, aggs, n)
 
     # KATs of the reference test-suite
     x = np.array([-1, -2, 0.5, 1.5, 4.5, 5], dtype="f8")

@@ -15,6 +15,19 @@ def load():
     return cases
 
 
+EDGES_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "edges_golden.npz")
+
+
+def load_edges():
+    """tests/golden/edges_golden.npz (tests/golden/make_golden_edges.py): the same case layout as binstats_golden.npz"""
+    z = np.load(EDGES_PATH, allow_pickle=False)
+    cases = {}
+    for key in z.files:
+        name, field = key.split("/", 1)
+        cases.setdefault(name, {})[field] = z[key]
+    return cases
+
+
 def binby_case(c):
     """-> (binners, aggs, n, expected) in the oracle's spec-dict form."""
     from oracle import oracle as O

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import golden_util
-from helpers import random_case, same
+from helpers import random_case, same, same_bits
 
 GOLD = golden_util.load()
 BINBY = sorted(k for k in GOLD if not k.startswith(("set_", "hash64")))
@@ -56,7 +56,56 @@ def test_oracle_matches_compiled_reference_random(seed, oracle, ref):
     want = ref.binby(binners, aggs, n)
     got = oracle.binby(binners, aggs, n)
     for a, w, g in zip(aggs, want, got):
-        assert same(np.asarray(w) if not np.ma.isMaskedArray(w) else w, g), (a["op"], None if a["data"] is None else a["data"].dtype)
+        assert same_bits(np.asarray(w) if not np.ma.isMaskedArray(w) else w, g), (a["op"], None if a["data"] is None else a["data"].dtype)
+
+
+@pytest.mark.parametrize("seed", range(40))
+def test_oracle_matches_compiled_reference_edges(seed, oracle, ref):
+    """the edge-value corpus (random_case(edges=True): integer limits, uint64 >= 2^63, +-0.0, +-inf, NaN payloads, subnormals,
+    overflowing powers, keys on bin edges, byte-swapped twins, moments 0..8, nunique), bit for bit"""
+    rng = np.random.default_rng(7000 + seed)
+    n = int(rng.integers(1, 3000))
+    binners, aggs = random_case(rng, n, edges=True)
+    want = ref.binby(binners, aggs, n)
+    got = oracle.binby(binners, aggs, n)
+    for a, w, g in zip(aggs, want, got):
+        assert same_bits(np.asarray(w) if not np.ma.isMaskedArray(w) else w, g), (a["op"], a.get("moment"), None if a["data"] is None else a["data"].dtype)
+
+
+EDGES = golden_util.load_edges()
+
+
+@pytest.mark.parametrize("name", sorted(EDGES))
+def test_oracle_matches_golden_edges(name, oracle):
+    """tests/golden/edges_golden.npz: edge-value cases and single-cell known answers from the compiled reference"""
+    binners, aggs, n, expected = golden_util.binby_case(EDGES[name])
+    got = oracle.binby(binners, aggs, n)
+    for a, w, g in zip(aggs, expected, got):
+        assert same_bits(w, g), (name, a["op"])
+
+
+def test_golden_edges_known_answers():
+    """the values the compiled reference gives for the cases where the device's rule is documented (DESIGN §3)"""
+    imin = np.iinfo(np.int64).min
+    assert EDGES["kat_moment3_int64_out_of_range"]["a0_result"].ravel()[2] == imin
+    assert EDGES["kat_moment3_uint64_out_of_range"]["a0_result"].ravel()[2] == 0
+    # 30000^4 + 30001^4 + 29999^4 + 1 = 2430000010800000003 exactly; the reference rounds its running sum through double
+    assert EDGES["kat_moment4_past_2p53"]["a0_result"].ravel()[2] == 2430000010800000000
+    r = EDGES["kat_minmax_signed_zeros"]
+    assert [np.signbit(r["a0_result"].ravel()[2]), np.signbit(r["a1_result"].ravel()[2])] == [True, True]
+
+
+def test_exact_sum_check_is_not_vacuous(oracle):
+    """helpers.float_sum_ok (the recursive-summation bound of the GPU tests) accepts the oracle and rejects a wrong cancelling sum"""
+    from helpers import float_sum_ok
+    v = np.array([1e16, 1.0, -1e16, 1.0])
+    b = [oracle.scalar(np.full(4, 0.5), 0, 1, 1)]
+    a = oracle.agg("sum", v)
+    w = oracle.binby(b, [a], 4)[0]
+    assert float_sum_ok(b, a, 4, w) is None
+    bad = w.copy()
+    bad.ravel()[2] = 100.0  # the bound here is gamma_4 * 2e16 ~ 9
+    assert float_sum_ok(b, a, 4, bad) is not None
 
 
 def test_oracle_first_mask_quirk_matches_reference(oracle, ref):

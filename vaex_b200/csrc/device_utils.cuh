@@ -119,6 +119,12 @@ __device__ __forceinline__ long long f64_to_i64_x86(double x) {
         return (long long)0x8000000000000000ULL;
     return __double2ll_rz(x);
 }
+// gcc's x86-64 double -> uint64 sequence: below 2^63 cvttsd2si as above, else cvttsd2si(x - 2^63) ^ 2^63; so >= 2^64 -> 0
+__device__ __forceinline__ unsigned long long f64_to_u64_x86(double x) {
+    if (x >= 9223372036854775808.0)
+        return (unsigned long long)f64_to_i64_x86(x - 9223372036854775808.0) ^ 0x8000000000000000ULL;
+    return (unsigned long long)f64_to_i64_x86(x);
+}
 
 // ---- BinnerScalar::to_bins, bit-exact (src/binners.cpp:13-57) -------------------------------------
 // scaled = (double(v) - vmin) * scale_v, scale_v = 1./(vmax-vmin) precomputed on the host in IEEE double.
@@ -220,6 +226,16 @@ __device__ __forceinline__ double pow_moment(double b, unsigned m) {
     }
     default: return pow(b, (double)m);
     }
+}
+// the same for integer grids, where the power is truncated to an integer: for m >= 5 repeated multiplication instead of pow
+// (pow may be 2 ulp off), exact while |b|^m < 2^53
+__device__ __forceinline__ double pow_moment_int(double b, unsigned m) {
+    if (m <= 4)
+        return pow_moment(b, m);
+    double r = b;
+    for (unsigned i = 1; i < m; i++)
+        r *= b;
+    return r;
 }
 
 // splitmix64 finaliser (src/hash.hpp:40-45)
