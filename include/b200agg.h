@@ -30,6 +30,7 @@
  *                         src/hash_primitives.cpp:45-56): update / merge / key_array / map_ordinal /
  *                         isin / create-from-keys, and hash<T> (src/hash.hpp:40-152).
  *   b200_minmax           the limits pre-pass: vaexfast statisticNd OP_MIN_MAX (src/vaexfast.cpp:1089-1101).
+ *   b200_stat_*           TaskPartStatistic + vaexfast statisticNd_f4/_f8, every op (vaex/cpu.py:487-626, src/vaexfast.cpp:1061-1278).
  *   b200_hash64           superutils.hash (src/superutils.cpp:265) — test hook, host only.
  */
 #ifndef B200AGG_H
@@ -240,6 +241,36 @@ int b200_set_counts(b200_set *set, int64_t *counts_out);
 /* out[0] = min, out[1] = max over non-NaN, unmasked values, as double; out = {+inf,-inf} when empty.
  */
 int b200_minmax(b200_ctx *ctx, int slot, int dtype, int byteswap, const void *data, const uint8_t *mask, int64_t nrows, int memspace, double *out);
+
+/* ---- legacy statistics: vaexfast statisticNd_f4 / _f8 (src/vaexfast.cpp:1061-1510) driven by TaskPartStatistic -------------
+ * (vaex/cpu.py:487-626): df.cov, df.correlation, binned df.minmax and the limits pre-pass.  Every column of a call is cast to the
+ * compute class `cls` (B200_F64 or B200_F32, chosen like vaex/cpu.py:527-541); a row masked in any column is dropped from every
+ * selection; selection masks are 1 byte per row, non-zero = the row takes part, a NULL entry = all rows.  b200_stat_read returns
+ * the reference's grid, double, C order (nselections, *sizes, fields) with the first binby dimension slowest; `sizes` already
+ * include the +3 of edges.  <= B200_MAX_BINNERS dimensions, <= B200_STAT_MAX_WEIGHTS weights (COV), <= B200_STAT_MAX_SELECTIONS.
+ * b200_stat_bin: `row_offset` is the global index of the call's first row.  FIRST breaks ties by (order, global row), so the calls
+ * of one pass must give every row its own index (chunk offsets of one row range).  DEVICE columns are read after the call returns:
+ * keep them alive until the slot's stream has finished (b200_ctx_sync, or b200_stat_read / reset / destroy, which wait for every
+ * slot). */
+#define B200_STAT_MAX_WEIGHTS 16
+#define B200_STAT_MAX_SELECTIONS 16
+typedef enum { B200_STAT_ADD1 = 0, B200_STAT_COUNT, B200_STAT_MIN_MAX, B200_STAT_MOMENTS_01,
+               B200_STAT_MOMENTS_012, B200_STAT_COV, B200_STAT_FIRST } b200_stat_op; /* = vaex.tasks OP_* codes */
+typedef struct {
+    const void *data;
+    int32_t dtype;       /* b200_dtype of `data` */
+    int32_t byteswap;    /* 1 = non-native byte order */
+    const uint8_t *mask; /* nullable, 1 = masked */
+} b200_stat_column;
+typedef struct b200_stat b200_stat;
+int b200_stat_create(b200_ctx *ctx, int op, int cls, int ndim, const int64_t *sizes, const double *minima, const double *maxima, int edges,
+                     int nweights, int nselections, b200_stat **out);
+int b200_stat_bin(b200_stat *stat, int slot, const b200_stat_column *binby, const b200_stat_column *weights, const uint8_t *const *selections,
+                  int64_t nrows, int64_t row_offset, int memspace, uint32_t flags);
+int b200_stat_fields(const b200_stat *stat);
+int b200_stat_read(b200_stat *stat, double *out);
+int b200_stat_reset(b200_stat *stat);
+int b200_stat_destroy(b200_stat *stat);
 
 /* ---- device-side expressions and filter compaction (SURVEY.md section 8f row 2) ------------------------------------------------
  * Replaces the per-chunk Python `eval` of virtual columns / filters / selections (vaex/scopes.py:108-128 _BlockScope.evaluate) and

@@ -2,7 +2,7 @@
 """Times every BASELINE.json configuration on one H100 with device-resident columns (the roofline setting) and prints one
 JSON object per config: rows/s, achieved algorithmic GB/s (SURVEY.md 8d bytes/row) and the fraction of the measured HBM peak.
 
-    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5]
+    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV]
 
 This is a companion to bench.py (which owns the headline line the driver parses); results are quoted in DESIGN.md.
 """
@@ -33,12 +33,19 @@ def main():
     stream = engine.slot_stream(ctx, 0)
     gen = torch.Generator(device="cuda").manual_seed(42)
 
-    def timed(fn, reps):
+    def timed(fn, reps, setup=None):
+        """best of `reps` device times of fn(); setup() (e.g. a grid reset) runs and finishes before each timed window"""
+        if setup:
+            setup()
         fn()
         ctx.sync()
         torch.cuda.synchronize()
         best = None
         for _ in range(reps):
+            if setup:
+                setup()
+                ctx.sync()
+                torch.cuda.synchronize()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(stream)
             fn()
@@ -71,6 +78,31 @@ def main():
             ms = timed(run, args.reps)
             assert int(a.get_result().sum()) == rows
             report("C1", "df.count(binby=x, shape=128) on 1e7 fp64 rows (shared-memory privatised)", rows, 8, ms)
+        elif cfg == "CV":
+            # legacy statistics (csrc/statistic.cu): (a) cov of 4 fp32 columns, no binby, 16 B/row; (b) the same on a 128^2 grid over two
+            # more fp32 columns, 24 B/row, a 5.2 MB reference grid of 40 fields; (c) OP_MIN_MAX of one fp64 column against b200_minmax
+            import ctypes as C
+            import subprocess
+            from vaex_b200 import statistic as ST
+            power = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+            cols = [torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen) for _ in range(6)]
+            for name, binby, sizes, bpr in (("CV-a", [], [], 16), ("CV-b", cols[4:], [128, 128], 24)):
+                st = ST.Statistic(ST.OP_COV.code, _lib.F32, sizes, [-3.0] * len(sizes), [3.0] * len(sizes), False, 4, 1, ctx=ctx)
+                ms = timed(lambda: st.bin(0, binby, cols[:4], [None], n, 0), args.reps, setup=st.reset)
+                report(name, "cov of 4 fp32 columns" + (" binby 2-D 128^2" if binby else ", no binby"), n, bpr, ms, gpu=power)
+                st.close()
+            del cols
+            torch.cuda.empty_cache()
+            x = torch.empty(n, dtype=torch.float64, device="cuda").normal_(generator=gen)
+            st = ST.Statistic(ST.OP_MIN_MAX.code, _lib.F64, [], [], [], False, 1, 1, ctx=ctx)
+            ms = timed(lambda: st.bin(0, [], [x], [None], n, 0), args.reps, setup=st.reset)
+            report("CV-c", "legacy OP_MIN_MAX of one fp64 column (k_stat_reg)", n, 8, ms, gpu=power)
+            st.close()
+            out = (C.c_double * 2)()
+            c = _lib.column(x)
+            ms = timed(lambda: _lib.check(_lib.lib().b200_minmax(ctx._h, 0, c.code, c.byteswap, c.ptr, None, c.length, c.memspace, out)), args.reps)
+            report("CV-c-minmax", "b200_minmax of the same column", n, 8, ms, gpu=power)
+            del x
         elif cfg in ("C5", "C2"):
             x = torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen)
             y = torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen)

@@ -8,6 +8,7 @@
 // each cell deposit its value.  Both passes recompute the flat index from the binner columns (cheaper than
 // materialising 8 B/row of indices).
 #include "binby_index.cuh"
+#include "cas128.cuh"
 
 namespace b200 {
 
@@ -15,44 +16,11 @@ namespace {
 
 constexpr int kThreads = 256;
 
-struct U128 {
-    unsigned long long lo, hi; // lo = order key, hi = global row
-};
-
-__device__ __forceinline__ U128 load_state(const unsigned long long *p) {
-    U128 v; // one 16-byte L2 load (never served from L1): the pair is read consistently enough for the CAS to validate
-    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(v.lo), "=l"(v.hi) : "l"(p) : "memory");
-    return v;
-}
-
-__device__ __forceinline__ U128 cas128(unsigned long long *addr, U128 cmp, U128 val) {
-    U128 old;
-    asm volatile("{\n\t"
-                 ".reg .b128 d, b, c;\n\t"
-                 "mov.b128 b, {%2, %3};\n\t"
-                 "mov.b128 c, {%4, %5};\n\t"
-                 "atom.global.cas.b128 d, [%6], b, c;\n\t"
-                 "mov.b128 {%0, %1}, d;\n\t"
-                 "}"
-                 : "=l"(old.lo), "=l"(old.hi)
-                 : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr)
-                 : "memory");
-    return old;
-}
-
-__device__ __forceinline__ bool less128(const U128 &a, const U128 &b) { return a.lo < b.lo || (a.lo == b.lo && a.hi < b.hi); }
-
 // monotone map of an order value to u64 so that `<` on the original type is `<` on the key; -0.0 == +0.0
 __device__ __forceinline__ unsigned long long order_key(int dt, uint64_t raw) {
     switch (dt) {
     case B200_F64:
-    case B200_F32: {
-        double d = raw_to_double(dt, raw);
-        if (d == 0.0)
-            d = 0.0;
-        unsigned long long b = (unsigned long long)__double_as_longlong(d);
-        return (b >> 63) ? ~b : (b | 0x8000000000000000ULL);
-    }
+    case B200_F32: return order_key_f64(raw_to_double(dt, raw));
     case B200_I64:
     case B200_I32:
     case B200_I16:
@@ -126,14 +94,7 @@ __global__ void __launch_bounds__(kThreads) k_first_select(const __grid_constant
         for (int j = 0; j < 4; j++) {
             if (!c[j].valid)
                 continue;
-            unsigned long long *st = p.state + 2 * idx[j];
-            U128 cur = load_state(st);
-            while (less128(c[j].kr, cur)) {
-                U128 old = cas128(st, cur, c[j].kr);
-                if (old.lo == cur.lo && old.hi == cur.hi)
-                    break;
-                cur = old;
-            }
+            cas128_min(p.state + 2 * idx[j], c[j].kr);
         }
     }
 }
@@ -161,7 +122,7 @@ __global__ void __launch_bounds__(kThreads) k_first_deposit(const __grid_constan
         for (int j = 0; j < 4; j++) {
             if (!c[j].valid)
                 continue;
-            U128 cur = load_state(p.state + 2 * idx[j]);
+            U128 cur = load128(p.state + 2 * idx[j]);
             if (cur.lo == c[j].kr.lo && cur.hi == c[j].kr.hi) { // exactly one row of the whole job matches
                 store_raw(p.grid, p.isz, idx[j], c[j].value_raw);
                 store_raw(p.order_grid, p.isz2, idx[j], c[j].order_raw);

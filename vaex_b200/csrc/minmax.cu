@@ -13,49 +13,10 @@
 #include <algorithm>
 
 #include "binby.cuh"
-#include "device_utils.cuh"
+#include "refvalue.cuh"
 
 namespace b200 {
 namespace {
-
-// the reference's cast + widening for one element of native type T
-template <typename T>
-__device__ __forceinline__ double ref_value(T v) {
-    return (double)(float)v; // numpy astype(float32): exact for <= 24-bit integers, round-to-nearest-even beyond
-}
-template <>
-__device__ __forceinline__ double ref_value<double>(double v) { return v; }
-template <>
-__device__ __forceinline__ double ref_value<float>(float v) { return (double)v; }
-template <>
-__device__ __forceinline__ double ref_value<long long>(long long v) { return __ll2double_rn(v); }
-template <>
-__device__ __forceinline__ double ref_value<unsigned long long>(unsigned long long v) { return (double)__ull2float_rn(v); }
-template <>
-__device__ __forceinline__ double ref_value<int>(int v) { return (double)__int2float_rn(v); }
-template <>
-__device__ __forceinline__ double ref_value<unsigned>(unsigned v) { return (double)__uint2float_rn(v); }
-
-template <typename T>
-__device__ __forceinline__ T swap_bytes(T v) {
-    if constexpr (sizeof(T) == 8) {
-        unsigned long long b;
-        memcpy(&b, &v, 8);
-        b = bswap(b, 8);
-        memcpy(&v, &b, 8);
-    } else if constexpr (sizeof(T) == 4) {
-        unsigned b;
-        memcpy(&b, &v, 4);
-        b = __byte_perm(b, 0, 0x0123);
-        memcpy(&v, &b, 4);
-    } else if constexpr (sizeof(T) == 2) {
-        unsigned short b;
-        memcpy(&b, &v, 2);
-        b = (unsigned short)((b >> 8) | (b << 8));
-        memcpy(&v, &b, 2);
-    }
-    return v;
-}
 
 constexpr int kThreads = 256;
 

@@ -8,6 +8,7 @@
 // reference's formula.  The table never overflows inside a kernel: the host sizes it for (pairs so far + rows of the batch)
 // before every launch and rehashes when it has to grow.
 #include "binby_index.cuh"
+#include "cas128.cuh"
 
 namespace b200 {
 
@@ -16,36 +17,11 @@ namespace {
 constexpr int kThreads = 256;
 constexpr unsigned long long kEmpty = ~0ull;
 
-struct U128 {
-    unsigned long long lo, hi; // lo = cell, hi = canonical value bits
-};
-
-__device__ __forceinline__ U128 load_pair(const unsigned long long *p) {
-    U128 v;
-    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(v.lo), "=l"(v.hi) : "l"(p) : "memory");
-    return v;
-}
-
-__device__ __forceinline__ U128 cas128(unsigned long long *addr, U128 cmp, U128 val) {
-    U128 old;
-    asm volatile("{\n\t"
-                 ".reg .b128 d, b, c;\n\t"
-                 "mov.b128 b, {%2, %3};\n\t"
-                 "mov.b128 c, {%4, %5};\n\t"
-                 "atom.global.cas.b128 d, [%6], b, c;\n\t"
-                 "mov.b128 {%0, %1}, d;\n\t"
-                 "}"
-                 : "=l"(old.lo), "=l"(old.hi)
-                 : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr)
-                 : "memory");
-    return old;
-}
-
 // true when (cell, canon) was not in the table yet
 __device__ __forceinline__ bool pair_insert(unsigned long long *table, unsigned long long mask, unsigned long long cell, unsigned long long canon) {
     unsigned long long h = hash64(canon ^ hash64(cell)) & mask;
     while (true) {
-        U128 cur = load_pair(table + 2 * h);
+        U128 cur = load128(table + 2 * h);
         if (cur.lo == kEmpty) {
             cur = cas128(table + 2 * h, U128{kEmpty, kEmpty}, U128{cell, canon});
             if (cur.lo == kEmpty)

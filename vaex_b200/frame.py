@@ -104,12 +104,128 @@ class Frame:
             min_value, count = int(lo), int(hi) - int(lo) + 1
         self.categories[name] = (int(min_value), int(count))
 
+    # ---- legacy statistics: TaskStatistic on the device (csrc/statistic.cu) ----------------------------------------------
+    def _statistic(self, op, binby, weights, limits, shape, selection, edges=False):
+        """TaskStatistic(self, binby, shape, limits, weights=weights, op=op, selection=selection) (vaex/tasks.py:431-470), run
+        through the executor; returns the reduced grid (one per selection when `selection` is a list)"""
+        binby = [] if binby is None else ([binby] if isinstance(binby, str) else list(binby))
+        shape = [shape] * len(binby) if np.isscalar(shape) else list(shape)
+        if limits is None or isinstance(limits, str):
+            limits = [None] * len(binby)
+        limits = list(limits)
+        if len(binby) == 1 and len(limits) == 2 and np.isscalar(limits[0]):
+            limits = [limits]
+        limits = [self.minmax(b).astype("float64") if lim is None else lim for b, lim in zip(binby, limits)]
+        waslist = isinstance(selection, (list, tuple))
+        selections = list(selection) if waslist else [selection]
+        masks = []
+        for one in selections:
+            if one is None or one is False:
+                masks.append(None)
+                continue
+            m = self.expression(one)
+            if m.dtype != np.bool_:
+                raise ValueError("a selection must be a boolean expression")
+            masks.append(m)
+        part = taskpart.TaskPartStatistic(self, [int(s) + 3 if edges else int(s) for s in shape], binby, np.dtype("f8"),
+                                          [None if m is None else "selection%d" % i for i, m in enumerate(masks)], op, list(weights),
+                                          [float(lim[0]) for lim in limits], [float(lim[1]) for lim in limits], edges, waslist)
+        columns = dict(self.columns)
+        for e in list(binby) + list(weights):
+            if e not in columns:
+                columns[e] = self.expression(e)
+        task = execution.Task(part, masks)
+        task.expressions = list(binby) + list(weights)
+        self.executor.execute(columns, [task], self.length, filter=self._filter)
+        return task.result
+
+    def cov(self, x, y=None, binby=None, limits=None, shape=128, selection=None):
+        """df.cov (vaex/dataframe.py:1402-1483): the covariance matrix of x and y, or of the expressions in the list x, from ONE
+        fused OP_COV pass; the last two dimensions are (N, N)"""
+        if y is None:
+            if not isinstance(x, (list, tuple)):
+                raise ValueError("if y argument is not given, x is expected to be sequence, not %r" % (x,))
+            expressions = list(x)
+        else:
+            expressions = [x, y]
+        from . import statistic as _stat
+        values = self._statistic(_stat.OP_COV, binby, expressions, limits, shape, selection)
+        N = len(expressions)
+        counts, sums = values[..., :N], values[..., N:2 * N]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            means = sums / counts
+        meansxy = means[..., None] * means[..., None, :]
+        shp = values.shape[:-1] + (N, N)
+        counts = values[..., 2 * N:2 * N + N**2].reshape(shp)
+        sums = values[..., 2 * N + N**2:].reshape(shp)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            moments2 = sums / counts
+        return moments2 - meansxy
+
+    def _correlation_matrix(self, column_names, binby=None, limits=None, shape=128, selection=None):
+        cov_matrix = self.cov(column_names, binby=binby, limits=limits, shape=shape, selection=selection)
+        diag = np.diagonal(cov_matrix, axis1=-2, axis2=-1)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            norm = (diag[..., np.newaxis, :] * diag[..., np.newaxis]) ** 0.5
+            return cov_matrix / norm
+
+    def correlation(self, x, y=None, binby=None, limits=None, shape=128, selection=None):
+        """df.correlation (vaex/dataframe.py:1302-1373): cov[x,y] / (std[x] std[y]); a list x without y gives the correlation matrix,
+        lists give arrays of pairwise results.  (The list-of-pairs form, which returns a DataFrame, is not provided.)"""
+        kw = dict(binby=binby, limits=limits, shape=shape, selection=selection)
+        seq = lambda v: isinstance(v, (list, tuple))  # noqa: E731
+        if y is None:
+            if not seq(x):
+                raise ValueError("if y not given, x is expected to be a list or tuple, not %r" % (x,))
+            if all(seq(k) and len(k) == 2 for k in x):
+                raise NotImplementedError("correlation of a list of pairs returns a vaex DataFrame; call it per pair")
+            return self._correlation_matrix(list(x), **kw)
+        if seq(x) and seq(y):
+            return np.array([[self.correlation(x_, y_, **kw) for y_ in y] for x_ in x])
+        if seq(x):
+            return np.array([self.correlation(x_, y, **kw) for x_ in x])
+        if seq(y):
+            return np.array([self.correlation(x, y_, **kw) for y_ in y])
+        return self._correlation_matrix([x, y], **kw)[..., 0, 1]
+
+    def covar(self, x, y, binby=None, limits=None, shape=128, selection=None):
+        """df.covar (vaex/dataframe.py:1248-1299): mean(x*y) - mean(x)*mean(y) through the binned aggregations, x*y a device
+        expression"""
+        single = not isinstance(x, (list, tuple))
+        xs, ys = ([x], [y]) if single else (list(x), list(y))
+        binby_l = [] if binby is None else ([binby] if isinstance(binby, str) else list(binby))
+        if binby_l and (limits is None or isinstance(limits, str)):
+            limits = [self.minmax(b).astype("float64") for b in binby_l]
+        out = []
+        for a, b in zip(xs, ys):
+            name = "(%s)*(%s)" % (a, b)
+            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
+            for e in (a, b):
+                if e not in f.columns:
+                    f.columns[e] = f.expression(e)
+            f.columns[name] = f.expression(name)
+            kw = dict(binby=binby_l or None, limits=limits, shape=shape, selection=selection)
+            mx, my, mxy = f._agg([_agg.mean(a), _agg.mean(b), _agg.mean(name)], **kw)
+            out.append(mxy - mx * my)
+        return out[0] if single else np.array(out)
+
     # ---- limits pre-pass ---------------------------------------------------------------------------------------------
-    def minmax(self, expression, raw=False):
+    def minmax(self, expression, raw=False, binby=None, limits=None, shape=128, selection=None):
         """df.minmax(expression): the limits pre-pass, on the device (csrc/minmax.cu).  Masked rows and NaN are ignored; like the
         reference (TaskStatistic(OP_MIN_MAX) over vaexfast.statisticNd, vaex/cpu.py:513-606) the reduction runs on the column cast
         to float64 (float64 / int64 columns) or float32 (everything else) and the (min, max) pair is cast back to the column dtype
-        (vaex/dataframe.py:1524-1528).  raw=True returns the two doubles of the statistic grid."""
+        (vaex/dataframe.py:1524-1528).  raw=True returns the two doubles of the statistic grid.
+        With `binby` (or a `selection`) the (min, max) pair is computed per bin through OP_MIN_MAX (csrc/statistic.cu); the last
+        dimension of the result is 2."""
+        if binby is not None or selection is not None:
+            from . import statistic as _stat
+            res = self._statistic(_stat.OP_MIN_MAX, binby, [expression], limits, shape, selection)
+            if raw:
+                return res
+            col = self.columns.get(expression)
+            dt = np.dtype(_dtype_of(col) if col is not None else self.expression(expression).dtype).newbyteorder("=")
+            with np.errstate(invalid="ignore"):
+                return res if dt.kind in "mM" else res.astype(dt)
         import ctypes as C
         col = self.columns[expression]
         ctx = _lib.context()

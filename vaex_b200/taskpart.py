@@ -15,6 +15,7 @@ from functools import reduce
 
 import numpy as np
 
+from . import _lib
 from . import agg as _agg
 from . import hash as _hash
 from . import superagg
@@ -291,6 +292,100 @@ class TaskPartHashmapUniqueCreate(TaskPart):
 
     def memory_usage(self):
         return self.hash_map_unique._internal.__sizeof__()
+
+
+class TaskPartStatistic(TaskPart):
+    """vaex/cpu.py:487-626 — the legacy statistics (df.cov, df.correlation, binned df.minmax, the limits pre-pass) on one device
+    grid per compute class (csrc/statistic.cu).  ``blocks`` are the binby blocks followed by the weight blocks."""
+    snake_name = "legacy_statistic"
+
+    def __init__(self, df, shape, expressions, dtype, selections, op, weights, minima, maxima, edges, selection_waslist):
+        self.df = df
+        self.shape = tuple(shape)
+        self.dtype = dtype
+        self.expressions = list(expressions)
+        self.op = op
+        self.weights = list(weights)
+        self.selections = list(selections)
+        self.fields = op.fields(weights)
+        self.shape_total = (len(self.selections),) + self.shape + (self.fields,)
+        self.minima = list(minima)
+        self.maxima = list(maxima)
+        self.edges = edges
+        self.selection_waslist = selection_waslist
+        self.stats = {}  # compute class -> _stat.Statistic, created on the first chunk of that class
+        self.grid = None
+
+    def get_bin_count(self):
+        return reduce(lambda a, b: a * b, self.shape, 1)
+
+    def ideal_splits(self, nthreads):
+        return 1  # one device grid shared by every thread
+
+    def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
+        from . import statistic as _stat
+        N = i2 - i1
+        if filter_mask is not None:  # the executor compacted the blocks with the filter
+            kept = getattr(filter_mask, "kept", None)
+            N = len(blocks[0]) if blocks else (int(kept) if kept is not None else int(np.asarray(filter_mask).sum()))
+        nd = len(self.expressions)
+        if not blocks and self.op.code != _stat.OP_ADD1.code:
+            raise ValueError("Nothing to compute for OP %s" % self.op.code)
+        for block in blocks[nd:]:
+            if _hash.is_string_column(block) or (not _is_device(block) and np.asarray(block).dtype.kind not in "biufmM"):
+                raise NotImplementedError("the legacy statistic of a string or object column has no GPU path")
+        dtypes = [np.dtype(block.__cuda_array_interface__["typestr"]) if _is_device(block) else block.dtype for block in blocks]
+        cls = _stat.compute_class(dtypes) if dtypes else _lib.F32
+        sels = []
+        for i, selection in enumerate(self.selections):
+            if selection is None or selection is False:
+                sels.append(None)
+                continue
+            mask = selection_masks[i]
+            if mask is None:
+                raise ValueError("performing operation on selection while no selection present")
+            if not _is_device(mask):
+                mask = np.asarray(mask.data & ~np.ma.getmaskarray(mask)) if np.ma.isMaskedArray(mask) else np.asarray(mask)  # unmask_selection_mask
+            sels.append(mask)
+        stat = self.stats.get(cls)
+        if stat is None:
+            stat = self.stats.setdefault(cls, _stat.Statistic(self.op.code, cls, self.shape, self.minima, self.maxima, self.edges,
+                                                              len(self.weights), len(self.selections)))
+        stat.bin(thread_index, blocks[:nd], blocks[nd:], sels, N, row_offset=i1)
+        return i2 - i1
+
+    def _grids(self):
+        if not self.stats:
+            grid = np.zeros(self.shape_total, np.float64)
+            self.op.init(grid)
+            return [grid]
+        return [s.read() for s in self.stats.values()]
+
+    def reduce(self, others):
+        # vaex/cpu.py:613-616: the op's own reduce over every grid (nansum / sum / nanmin+nanmax / argmin of the order)
+        grids = self._grids() + [g for o in others for g in o._grids()]
+        dtype = np.dtype(getattr(self.dtype, "numpy", self.dtype))
+        self.grid = self.op.reduce(np.array(grids).astype(dtype, copy=False))
+        for s in self.stats.values():
+            s.close()
+        self.stats = {}
+
+    def get_result(self):
+        if self.grid is None:
+            self.reduce([])
+        return self.grid if self.selection_waslist else self.grid[0]
+
+    @classmethod
+    def decode(cls, encoding, spec, df=None, nthreads=1):
+        """``spec`` = TaskStatistic.encode() (vaex/tasks.py:409-413); without an ``encoding`` the '_op' spec is decoded locally"""
+        from . import statistic as _stat
+        spec = dict(spec)
+        if encoding is not None:
+            spec["op"] = encoding.decode("_op", spec["op"])
+            spec["dtype"] = encoding.decode("dtype", spec["dtype"])
+        elif isinstance(spec["op"], dict):
+            spec["op"] = _stat.decode_op(spec["op"])
+        return cls(df, **spec)
 
 
 REGISTRY = {cls.snake_name: cls for cls in (TaskPartAggregation, TaskPartHashmapUniqueCreate)}

@@ -76,16 +76,32 @@ class VaexTaskPartHashmapUniqueCreate(_tp.TaskPartHashmapUniqueCreate):
         return super().process(thread_index, i1, i2, filter_mask, selection_masks, blocks)
 
 
+class VaexTaskPartStatistic(_tp.TaskPartStatistic):
+    """"legacy_statistic" (vaex/cpu.py:487-626): TaskStatistic — df.cov / df.correlation / binned df.minmax and the limits pre-pass of
+    df.count(binby=..., limits=None) (vaex/dataframe.py:1519-1521)."""
+    snake_name = "legacy_statistic"
+
+    def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
+        import vaex.array_types
+        blocks = [vaex.array_types.to_numpy(b, strict=False) for b in blocks]
+        sel = [None if s is None else vaex.array_types.to_numpy(s) for s in selection_masks]
+        return super().process(thread_index, i1, i2, filter_mask, sel, blocks)
+
+
 _ORIGINAL = {}
 
 
-def install():
-    """Swap the two task parts in vaex's registry; returns the replaced classes so `uninstall` can restore them."""
+def install(legacy_statistic=False):
+    """Swap the two task parts in vaex's registry — and with ``legacy_statistic=True`` also "legacy_statistic" (TaskStatistic);
+    returns the replaced classes so `uninstall` can restore them."""
     import vaex.cpu
     _ORIGINAL["aggregations"] = vaex.cpu.TaskPartAggregation
     _ORIGINAL["hash_map_unique_create"] = vaex.cpu.TaskPartHashmapUniqueCreate
     vaex.cpu.register(VaexTaskPartAggregation)
     vaex.cpu.register(VaexTaskPartHashmapUniqueCreate)
+    if legacy_statistic:
+        _ORIGINAL["legacy_statistic"] = vaex.cpu.TaskPartStatistic
+        vaex.cpu.register(VaexTaskPartStatistic)
     return dict(_ORIGINAL)
 
 
