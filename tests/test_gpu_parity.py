@@ -159,9 +159,10 @@ def test_tile_partitioned_count_matches_oracle(oracle):
 
 @pytest.mark.parametrize("case", ["2d_f32_sorted_keys", "1d_f64_64parts", "3d_f32_128parts", "2d_f64_two_hot_parts", "2d_f32_all_nan_y", "2d_f32_ragged"])
 def test_ring_partition_variants(case, oracle):
-    """csrc/ringcount.cu over its template space (fp32 / fp64 keys, 1-3 dimensions, 32 / 64 / 128 parts) and the distributions
-    that stress the rings and the chunk lists: keys sorted by the partitioning dimension (every warp fills ONE ring: overflow ->
-    direct REDs), two hot parts, a column of NaN (everything in cell row 0), a row count that is no multiple of anything."""
+    """csrc/ringcount.cu over its template space (fp32 / fp64 keys, 1-3 dimensions, 32 / 64 parts) and the distributions that
+    stress the rings and the chunk lists: keys sorted by the partitioning dimension (every warp fills ONE ring: overflow -> direct
+    REDs), two hot parts, a column of NaN (everything in cell row 0), a row count that is no multiple of anything.  The 3-D case's
+    grids (160^3 and 153^3 cells) are above the ring's 64 x 49,151 cells: the direct kernel counts them."""
     rng = np.random.default_rng(77)
     n = (1 << 22) + 4097
     if case == "2d_f32_sorted_keys":

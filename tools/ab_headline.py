@@ -4,7 +4,7 @@
     VAEX_B200_LIB=/path/to/other/libb200agg.so python tools/ab_headline.py [--rows 1e9] [--reps 10]
 
 Box-to-box variation between gpurun calls is ~5 % (the same unchanged kernel differs that much), so kernel variants are only
-compared inside one call: run this script once per library build / environment knob.  Prints one JSON line."""
+compared inside one call: run this script once per library build.  Prints one JSON line."""
 import argparse
 import json
 import os
@@ -57,7 +57,7 @@ def main():
     import hashlib
     sha = hashlib.sha1(res.tobytes()).hexdigest()[:16]
     times.sort()
-    print(json.dumps({"tag": args.tag, "lib": os.path.basename(_lib.LIB_PATH), "path": "ring", "fg": os.environ.get("B200_RING_FG"), "rows": n, "occupy": args.occupy or None,
+    print(json.dumps({"tag": args.tag, "lib": os.path.basename(_lib.LIB_PATH), "path": "ring", "rows": n, "occupy": args.occupy or None,
                       "ms_min": times[0], "ms_median": times[len(times) // 2], "rows_per_s_median": n / (times[len(times) // 2] * 1e-3), "count_ok": total == n, "grid_sha": sha}))
 
 

@@ -15,8 +15,6 @@
 //
 // Bound: the scatter.  Large grids issue one L2 RED per row per aggregator; L1TEX/LSU retires ~1 scattered lane
 // per clock per SM, so rows/s <= 132 SMs x f_SM / n_aggs — well below the HBM stream rate for 8-12 B rows.
-#include <stdlib.h>
-
 #include "binby_index.cuh"
 
 namespace b200 {
@@ -234,53 +232,120 @@ __global__ void k_merge(int op, int cell_dtype, void *dst, const void *src, uint
     }
 }
 
-template <bool VEC, bool SMEM>
-int launch_variant(b200_ctx *ctx, cudaStream_t stream, const BinParams &p) {
-    size_t smem = SMEM ? (size_t)p.smem_copies * p.smem_copy_bytes : 0;
-    auto kern = k_binby<VEC, SMEM>;
-    if (smem > 48 * 1024)
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-    if (per_sm < 1)
-        per_sm = 1;
-    long long want = (p.nrows + (long long)kThreads * 4 - 1) / ((long long)kThreads * 4);
-    long long cap = (long long)ctx->sm_count * per_sm;
-    int blocks = (int)(want < cap ? want : cap);
-    if (blocks < 1)
-        blocks = 1;
-    kern<<<blocks, kThreads, smem, stream>>>(p);
-    B200_CUDA(cudaGetLastError());
-    return B200_OK;
+// The float plan of a call (FloatPlan); false when a binner or an aggregator is outside what the float-key kernels handle.
+// count(*) reads no column, so its byte order does not matter.
+bool float_plan(const BinParams &bp, FloatPlan *f) {
+    if (bp.nb < 1 || bp.nb > 3 || bp.na < 1 || bp.cells >= (1ull << 32))
+        return false;
+    memset(f, 0, sizeof *f);
+    FastParams &p = f->p;
+    f->xdtype = bp.b[0].dtype;
+    f->nd = bp.nb;
+    f->vdtype = -1;
+    if (f->xdtype != B200_F32 && f->xdtype != B200_F64)
+        return false;
+    for (int i = 0; i < bp.nb; i++) {
+        const DevBinner &b = bp.b[i];
+        if (b.kind != B200_BINNER_SCALAR || b.dtype != f->xdtype || b.byteswap || b.mask || b.bins < 1 || b.bins >= (1ull << 30))
+            return false;
+        p.x[i] = b.data;
+        p.vmin[i] = b.vmin;
+        p.scale[i] = b.scale;
+        p.bins_d[i] = b.bins_d;
+        p.bins[i] = (unsigned)b.bins;
+        p.stride[i] = (unsigned)b.stride;
+    }
+    for (int k = 0; k < bp.na; k++) {
+        const DevAgg &a = bp.a[k];
+        if (a.mask)
+            return false;
+        if (a.op == B200_AGG_COUNT && !a.data) {
+            if (p.count_star)
+                return false;
+            p.count_star = static_cast<unsigned long long *>(a.grid);
+            continue;
+        }
+        if (a.byteswap || (a.dtype != B200_F32 && a.dtype != B200_F64))
+            return false;
+        if (p.v && (p.v != a.data || f->vdtype != a.dtype))
+            return false; // one value column only
+        p.v = a.data;
+        f->vdtype = a.dtype;
+        if (a.op == B200_AGG_COUNT && !p.vcount)
+            p.vcount = static_cast<unsigned long long *>(a.grid);
+        else if (a.op == B200_AGG_SUM && !p.vsum)
+            p.vsum = static_cast<double *>(a.grid);
+        else if (a.op == B200_AGG_SUM_MOMENT && a.moment == 2 && !p.vm2)
+            p.vm2 = static_cast<double *>(a.grid);
+        else
+            return false;
+    }
+    p.nrows = bp.nrows;
+    p.cells = (unsigned)bp.cells;
+    return true;
 }
 
 } // namespace
 
-int try_launch_fast(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool vec, bool *taken);          // fast.cu
-int try_launch_ringcount(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool vec, bool *taken);     // ringcount.cu
-
-int launch_binby(b200_ctx *ctx, Slot *slot, const BinParams &p, bool vec) {
-    if (p.nrows <= 0)
+int slot_scratch(Slot *slot, size_t need, bool *room) {
+    *room = true;
+    if (slot->scratch_cap >= need)
         return B200_OK;
-    if (p.nrows >= (1ll << 38)) { // the shared-memory sub-histograms count in 32 bits per CTA: >= 132 CTAs keep a CTA's share below 2^31
-        set_error("b200_bin: %lld rows in one call (the limit is 2^38; an H100 holds < 2^38 rows of any column)", (long long)p.nrows);
+    if (slot->scratch) {
+        B200_CUDA(cudaStreamSynchronize(slot->stream));
+        B200_CUDA(cudaFree(slot->scratch));
+        slot->scratch = nullptr;
+        slot->scratch_cap = 0;
+    }
+    if (cudaMalloc(&slot->scratch, need) != cudaSuccess) {
+        cudaGetLastError();
+        *room = false;
+        return B200_OK;
+    }
+    slot->scratch_cap = need;
+    return B200_OK;
+}
+
+// The one place that picks the kernel of a b200_bin call: the ring pair, the float-key kernel with shared-memory copies, the
+// region sort, the float-key kernel with global REDs, else the descriptor-driven k_binby.
+int launch_binby(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool vec) {
+    if (bp.nrows <= 0)
+        return B200_OK;
+    if (bp.nrows >= (1ll << 38)) { // the shared-memory sub-histograms count in 32 bits per CTA: >= 132 CTAs keep a CTA's share below 2^31
+        set_error("b200_bin: %lld rows in one call (the limit is 2^38; an H100 holds < 2^38 rows of any column)", (long long)bp.nrows);
         return B200_ERR_INVALID;
     }
-    cudaStream_t stream = slot->stream;
-    // B200_DISABLE_FAST=1 forces the descriptor-driven kernel (A/B measurements, parity tests of both kernels)
-    static const bool disable_fast = getenv("B200_DISABLE_FAST") && atoi(getenv("B200_DISABLE_FAST")) != 0;
-    if (!disable_fast) {
-        bool taken = false;
-        B200_CHECK(try_launch_ringcount(ctx, slot, p, vec, &taken));
-        if (taken)
-            return B200_OK;
-        B200_CHECK(try_launch_fast(ctx, slot, p, vec, &taken));
+    FloatPlan f;
+    if (!vec || !float_plan(bp, &f)) {
+        const bool smem = bp.smem_copies > 0;
+        auto kern = smem ? (vec ? k_binby<true, true> : k_binby<false, true>) : (vec ? k_binby<true, false> : k_binby<false, false>);
+        return launch_persistent(ctx, slot->stream, kern, kThreads, smem ? (size_t)bp.smem_copies * bp.smem_copy_bytes : 0, kThreads * 4, bp);
+    }
+    FastParams &p = f.p;
+    const unsigned long long cells = bp.cells;
+    bool taken = false;
+    // count(*) of >= 2^22 rows on a grid too big for shared-memory copies, small enough for <= kRingParts parts: the ring pair
+    if (p.count_star && !p.v && bp.nrows >= (1ll << 22) && cells * 4 > 96 * 1024 && cells <= (unsigned long long)kRingTileCells * kRingParts &&
+        cells < (1ull << 22)) {
+        B200_CHECK(launch_ringcount(ctx, slot, f, &taken));
         if (taken)
             return B200_OK;
     }
-    if (p.smem_copies > 0)
-        return vec ? launch_variant<true, true>(ctx, stream, p) : launch_variant<false, true>(ctx, stream, p);
-    return vec ? launch_variant<true, false>(ctx, stream, p) : launch_variant<false, false>(ctx, stream, p);
+    // shared-memory privatisation for small grids (shared-memory atomics retire several times more lanes per clock than L2 REDs)
+    size_t copy = ((p.vsum ? 8ull : 0) + (p.vm2 ? 8ull : 0) + (p.count_star ? 4ull : 0) + (p.vcount ? 4ull : 0)) * cells;
+    copy = (copy + 15) / 16 * 16;
+    if (copy <= 96 * 1024 && bp.nrows >= 8192) {
+        p.smem_copies = std::min(std::max((int)(32 * 1024 / copy), 1), 8);
+        return launch_fast(ctx, slot->stream, f, copy * p.smem_copies);
+    }
+    // accumulators larger than the L2: sort the rows by grid region first, when the input is big enough to pay for it
+    const int naggs = (p.count_star != nullptr) + (p.vcount != nullptr) + (p.vsum != nullptr) + (p.vm2 != nullptr);
+    if (((size_t)naggs * 8 * cells > ctx->l2_bytes || getenv("B200_TILESORT_FORCE")) && bp.nrows >= env_ll("B200_TILESORT_MIN_ROWS", 1ll << 24)) {
+        B200_CHECK(launch_tilesort(ctx, slot, f, &taken));
+        if (taken)
+            return B200_OK;
+    }
+    return launch_fast(ctx, slot->stream, f, 0);
 }
 
 int launch_fill(cudaStream_t stream, void *ptr, int cell_dtype, uint64_t cells, uint64_t bits) {

@@ -1,5 +1,10 @@
 // binby.cuh — kernel parameter blocks shared by the binby kernels and the C-ABI layer.
 #pragma once
+#include <stdlib.h>
+
+#include <algorithm>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace b200 {
@@ -62,12 +67,17 @@ struct FirstParams {
     uint8_t *cell_masked;
 };
 
-// specialised float-binner paths (fast.cu, tilesort.cu)
-struct FastParams {
+// ---- specialised float-key paths (ringcount.cu, fast.cu, tilesort.cu), picked by launch_binby --------------------------------
+// 1-3 scalar binners over one float type, native byte order, no masks.  The first 120 bytes of FastParams and RingParams: no
+// padding, so the kernels' parameter offsets are those of the flat structs this replaced.
+struct FloatKeys {
     const void *x[3];
     double vmin[3], scale[3], bins_d[3];
     unsigned bins[3];
     unsigned stride[3];
+};
+
+struct FastParams : FloatKeys {
     long long nrows;
     unsigned cells;
     const void *v;                      // value column or null
@@ -78,8 +88,59 @@ struct FastParams {
     int smem_copies;                    // > 0: privatise in shared memory (u32 counts, f64 sums)
 };
 
-// tilesort.cu: rows sorted by grid region first, so that the scatter works on an L2-resident part of the grids
-int try_launch_tilesort(b200_ctx *ctx, Slot *slot, const FastParams &p, int xdtype, int nd, int vdtype, bool *taken);
+// a b200_bin call the float-key kernels can take: keys, count(*) / count(v) / sum(v) / sum(v^2) of at most one value column
+struct FloatPlan {
+    FastParams p;
+    int xdtype; // B200_F32 / B200_F64, every key column
+    int nd;     // key columns, 1..3
+    int vdtype; // of the value column, -1 without one
+};
+
+// ringcount.cu: parts of <= kRingTileCells cells (192 KB of u32 counters in k_ring_count, one of them the pad cell), <= kRingParts
+constexpr unsigned kRingTileCells = 49151;
+constexpr int kRingParts = 64;
+
+// Each launches one variant for the plan.  The ring pair and the region sort set *taken = false, with no error, when their
+// scratch or part geometry does not work out for this grid: the caller then takes the next kernel.
+int launch_ringcount(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken);
+int launch_fast(b200_ctx *ctx, cudaStream_t stream, const FloatPlan &f, size_t smem);
+int launch_tilesort(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken);
+
+// Calls fn(T(), std::integral_constant<int, ND>()) with the plan's key type (float / double) and dimension count.
+template <typename F>
+int with_keys(const FloatPlan &f, F &&fn) {
+    auto nd = [&](auto t) {
+        switch (f.nd) {
+        case 1: return fn(t, std::integral_constant<int, 1>());
+        case 2: return fn(t, std::integral_constant<int, 2>());
+        default: return fn(t, std::integral_constant<int, 3>());
+        }
+    };
+    return f.xdtype == B200_F32 ? nd(float()) : nd(double());
+}
+
+// Grid-stride kernels: one CTA per `rows_per_cta` rows, at most as many as are resident on all SMs at once.
+template <typename P>
+int launch_persistent(b200_ctx *ctx, cudaStream_t stream, void (*kern)(P), int threads, size_t smem, long long rows_per_cta, const P &p) {
+    if (smem > 48 * 1024)
+        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    const long long want = (p.nrows + rows_per_cta - 1) / rows_per_cta, cap = (long long)ctx->sm_count * std::max(per_sm, 1);
+    kern<<<(int)std::max(std::min(want, cap), 1ll), threads, smem, stream>>>(p);
+    B200_CUDA(cudaGetLastError());
+    return B200_OK;
+}
+
+// tuning knobs of the region sort, read per call (tests shrink them to reach every variant with small inputs)
+inline long long env_ll(const char *name, long long dflt) {
+    const char *e = getenv(name);
+    return e && *e ? atoll(e) : dflt;
+}
+
+// Grows slot->scratch (partition scratch) to at least `need` bytes; the old block is freed once the slot's stream has drained.
+// *room = false, with no error set, when cudaMalloc refuses: the caller then takes another kernel.
+int slot_scratch(Slot *slot, size_t need, bool *room);
 
 // NUNIQUE (nunique.cu)
 struct NUniqueParams {

@@ -10,6 +10,22 @@ __device__ __forceinline__ uint4 ldcs128(const void *p) { return __ldcs(reinterp
 __device__ __forceinline__ uint2 ldcs64(const void *p) { return __ldcs(reinterpret_cast<const uint2 *>(p)); }
 __device__ __forceinline__ unsigned ldcs32(const void *p) { return __ldcs(reinterpret_cast<const unsigned *>(p)); }
 
+// 4 consecutive elements of a float / double column from element i (16-byte aligned): one or two 128-bit loads
+template <typename T>
+__device__ __forceinline__ void ldcs4(const void *p, long long i, T out[4]);
+template <>
+__device__ __forceinline__ void ldcs4<float>(const void *p, long long i, float out[4]) {
+    const uint4 a = ldcs128(static_cast<const float *>(p) + i);
+    out[0] = __uint_as_float(a.x), out[1] = __uint_as_float(a.y), out[2] = __uint_as_float(a.z), out[3] = __uint_as_float(a.w);
+}
+template <>
+__device__ __forceinline__ void ldcs4<double>(const void *p, long long i, double out[4]) {
+    const uint4 *q = reinterpret_cast<const uint4 *>(static_cast<const double *>(p) + i);
+    const uint4 a = __ldcs(q), b = __ldcs(q + 1);
+    out[0] = __longlong_as_double(((long long)a.y << 32) | a.x), out[1] = __longlong_as_double(((long long)a.w << 32) | a.z);
+    out[2] = __longlong_as_double(((long long)b.y << 32) | b.x), out[3] = __longlong_as_double(((long long)b.w << 32) | b.z);
+}
+
 __device__ __forceinline__ uint64_t bswap(uint64_t v, int isz) {
     switch (isz) {
     case 8: {

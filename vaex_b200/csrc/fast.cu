@@ -8,20 +8,16 @@
 // 64-bit index math.  The bound that remains is the scatter itself: one RED per row per aggregator, retired by the L2 at a
 // fixed chip-wide rate whatever the operand width.
 //
-// Load pattern: each thread owns ROWS = 32/sizeof(T) consecutive... no — two 128-bit loads per column per step, the second
-// one 32 lanes further on, so every warp-level LDG.128 is a dense 512-byte segment (fully coalesced, evict-first).
-#include <stdlib.h>
-
+// Load pattern: two 128-bit loads per column per step, the second one 32 lanes further on, so every warp-level LDG.128 is a
+// dense 512-byte segment (fully coalesced, evict-first).
 #include "binby.cuh"
 #include "device_utils.cuh"
 
 namespace b200 {
 
-
 namespace {
 
 constexpr int kThreads = 256;
-
 
 template <typename T>
 __device__ __forceinline__ double widen(T v);
@@ -30,7 +26,8 @@ __device__ __forceinline__ double widen<float>(float v) { return (double)v; }
 template <>
 __device__ __forceinline__ double widen<double>(double v) { return v; }
 
-// R consecutive elements starting at element index i (16-byte aligned): R = 4 for float, 2 for double
+// R consecutive elements starting at element index i (16-byte aligned): R = 4 for float, 2 for double.  One 128-bit load per
+// column and half-step whatever T (ldcs4 reads 4 doubles with two), so that both loads of a warp are dense 512-byte segments.
 template <typename T>
 struct Vec;
 template <>
@@ -201,120 +198,23 @@ __global__ void __launch_bounds__(kThreads) k_binby_fast(const __grid_constant__
     }
 }
 
-template <typename T, int ND, typename TV, bool HASV>
-int launch3(b200_ctx *ctx, cudaStream_t stream, const FastParams &p, size_t smem) {
-    auto go = [&](auto kern) -> int {
-        if (smem > 48 * 1024)
-            B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        B200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
-        if (per_sm < 1)
-            per_sm = 1;
-        const long long rows_per_cta = (long long)kThreads * 2 * Vec<T>::R;
-        long long want = (p.nrows + rows_per_cta - 1) / rows_per_cta;
-        long long cap = (long long)ctx->sm_count * per_sm;
-        int blocks = (int)(want < cap ? want : cap);
-        kern<<<blocks < 1 ? 1 : blocks, kThreads, smem, stream>>>(p);
-        B200_CUDA(cudaGetLastError());
-        return B200_OK;
-    };
-    if (p.smem_copies > 0)
-        return go(k_binby_fast<T, ND, TV, HASV, true>);
-    return go(k_binby_fast<T, ND, TV, HASV, false>);
-}
-
-template <typename T, int ND>
-int launch2(b200_ctx *ctx, cudaStream_t stream, const FastParams &p, int vdtype, size_t smem) {
-    if (!p.v)
-        return launch3<T, ND, float, false>(ctx, stream, p, smem);
-    if (vdtype == B200_F32)
-        return launch3<T, ND, float, true>(ctx, stream, p, smem);
-    return launch3<T, ND, double, true>(ctx, stream, p, smem);
-}
-
-template <typename T>
-int launch1(b200_ctx *ctx, cudaStream_t stream, const FastParams &p, int nd, int vdtype, size_t smem) {
-    switch (nd) {
-    case 1: return launch2<T, 1>(ctx, stream, p, vdtype, smem);
-    case 2: return launch2<T, 2>(ctx, stream, p, vdtype, smem);
-    default: return launch2<T, 3>(ctx, stream, p, vdtype, smem);
-    }
-}
-
 } // namespace
 
-// Returns B200_OK and sets *taken when the request matched the fast path and was launched.
-int try_launch_fast(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool vec, bool *taken) {
-    cudaStream_t stream = slot->stream;
-    *taken = false;
-    if (!vec || bp.nb < 1 || bp.nb > 3 || bp.na < 1 || bp.cells >= (1ull << 32) || bp.nrows <= 0)
-        return B200_OK;
-    FastParams p;
-    memset(&p, 0, sizeof p);
-    const int t = bp.b[0].dtype;
-    if (t != B200_F32 && t != B200_F64)
-        return B200_OK;
-    for (int i = 0; i < bp.nb; i++) {
-        const DevBinner &b = bp.b[i];
-        if (b.kind != B200_BINNER_SCALAR || b.dtype != t || b.byteswap || b.mask || b.bins < 1 || b.bins >= (1ull << 30))
-            return B200_OK;
-        p.x[i] = b.data;
-        p.vmin[i] = b.vmin;
-        p.scale[i] = b.scale;
-        p.bins_d[i] = b.bins_d;
-        p.bins[i] = (unsigned)b.bins;
-        p.stride[i] = (unsigned)b.stride;
-    }
-    int vdtype = -1;
-    for (int k = 0; k < bp.na; k++) {
-        const DevAgg &a = bp.a[k];
-        if (a.mask || a.byteswap)
-            return B200_OK;
-        if (a.op == B200_AGG_COUNT && !a.data) {
-            if (p.count_star)
-                return B200_OK;
-            p.count_star = static_cast<unsigned long long *>(a.grid);
-            continue;
-        }
-        if (a.dtype != B200_F32 && a.dtype != B200_F64)
-            return B200_OK;
-        if (p.v && (p.v != a.data || vdtype != a.dtype))
-            return B200_OK; // one value column only
-        p.v = a.data;
-        vdtype = a.dtype;
-        if (a.op == B200_AGG_COUNT && !p.vcount)
-            p.vcount = static_cast<unsigned long long *>(a.grid);
-        else if (a.op == B200_AGG_SUM && !p.vsum)
-            p.vsum = static_cast<double *>(a.grid);
-        else if (a.op == B200_AGG_SUM_MOMENT && a.moment == 2 && !p.vm2)
-            p.vm2 = static_cast<double *>(a.grid);
-        else
-            return B200_OK;
-    }
-    p.nrows = bp.nrows;
-    p.cells = (unsigned)bp.cells;
-    // shared-memory privatisation for small grids (shared-memory atomics retire several times more lanes per clock than L2 REDs)
-    size_t copy = ((p.vsum ? 8ull : 0) + (p.vm2 ? 8ull : 0) + (p.count_star ? 4ull : 0) + (p.vcount ? 4ull : 0)) * bp.cells;
-    copy = (copy + 15) / 16 * 16;
-    size_t smem = 0;
-    if (copy <= 96 * 1024 && bp.nrows >= 8192) {
-        int copies = (int)(32 * 1024 / copy);
-        p.smem_copies = copies < 1 ? 1 : (copies > 8 ? 8 : copies);
-        smem = copy * p.smem_copies;
-    }
-    const int naggs = (p.count_star != nullptr) + (p.vcount != nullptr) + (p.vsum != nullptr) + (p.vm2 != nullptr);
-    if (!smem && ((size_t)naggs * 8 * bp.cells > ctx->l2_bytes || getenv("B200_TILESORT_FORCE"))) {
-        // accumulators larger than the L2: sort the rows by grid region first (tilesort.cu), when the input is big enough to pay for it
-        bool sorted = false;
-        B200_CHECK(try_launch_tilesort(ctx, slot, p, t, bp.nb, vdtype, &sorted));
-        if (sorted) {
-            *taken = true;
-            return B200_OK;
-        }
-    }
-    *taken = true;
-    int rc = t == B200_F32 ? launch1<float>(ctx, stream, p, bp.nb, vdtype, smem) : launch1<double>(ctx, stream, p, bp.nb, vdtype, smem);
-    return rc;
+// smem > 0: f.p.smem_copies private copies of that many bytes in all
+int launch_fast(b200_ctx *ctx, cudaStream_t stream, const FloatPlan &f, size_t smem) {
+    return with_keys(f, [&](auto t, auto nd) {
+        using T = decltype(t);
+        constexpr int ND = decltype(nd)::value;
+        auto go = [&](auto tv, auto hasv) {
+            using TV = decltype(tv);
+            constexpr bool HASV = decltype(hasv)::value;
+            auto kern = smem ? k_binby_fast<T, ND, TV, HASV, true> : k_binby_fast<T, ND, TV, HASV, false>;
+            return launch_persistent(ctx, stream, kern, kThreads, smem, kThreads * 2 * Vec<T>::R, f.p);
+        };
+        if (!f.p.v)
+            return go(float(), std::false_type());
+        return f.vdtype == B200_F32 ? go(float(), std::true_type()) : go(double(), std::true_type());
+    });
 }
 
 } // namespace b200

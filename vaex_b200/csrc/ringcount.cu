@@ -6,9 +6,7 @@
 // cut into <= 32 (else 64) GRID TILES ("parts") of <= 49152 consecutive cells and the rows are partitioned by part first:
 //
 //   K1 k_ring_partition  every WARP is autonomous.  The keys of the NEXT 256-row group are loaded into registers (128-bit,
-//                        evict-first loads) while the current group is placed; a TMA-staged variant (cp.async.bulk + mbarrier,
-//                        double buffered) spends warp instructions on issuing the bulk copies and 4 KB of shared memory per
-//                        warp on the buffers.
+//                        evict-first loads) while the current group is placed.
 //                        Per row: the bit-exact fp64 bin index, part = idx / tile_cells (one IMAD.HI), ONE shared-memory atomic
 //                        on the (warp, part) counter whose return value is the row's slot in that part's RING (96 entries), and
 //                        one 16-bit store of the local cell index into the ring.  Every 256 rows the rings that hold a full
@@ -38,11 +36,7 @@
 
 namespace b200 {
 
-struct RingParams {
-    const void *x[3];
-    double vmin[3], scale[3], bins_d[3];
-    unsigned bins[3];
-    unsigned stride[3];
+struct RingParams : FloatKeys {
     unsigned stride_sum;          // sum(stride): bin_cell_m1 returns cell - 1
     float clamp_lo[3], clamp_hi[3]; // CLAMPED variant (fp32 keys): see bin_cell_m2_clamped
     long long row0, nrows;        // this batch
@@ -68,31 +62,11 @@ namespace {
 
 constexpr int kGroupRows = 256;   // rows between two ring flushes: 8 per lane
 constexpr int kGran = 16;         // entries per lane and step in k_ring_count
-#ifndef B200_RING_LINE
-#define B200_RING_LINE 64
-#endif
-constexpr unsigned kLine = B200_RING_LINE; // entries a ring flush moves: 32 = 64 bytes (two sectors), 64 = one 128-byte line
-constexpr int kLineLanes = kLine / 8;      // lanes that move one line with 16 bytes each
+constexpr unsigned kLine = 64;    // entries a ring flush moves: one 128-byte line
+constexpr int kLineLanes = kLine / 8; // lanes that move one line with 16 bytes each
 constexpr unsigned kSuper = 32;   // chunks a warp reserves from the pool at a time
-constexpr unsigned kMaxTileCells = 49151; // 192 KB of u32 counters in k_ring_count, one of them the pad cell
-constexpr int kMaxParts = 64;
 constexpr unsigned kNone = 0xFFFFFFFFu;
 constexpr int kCountThreads = 1024;
-
-template <typename T>
-__device__ __forceinline__ void ldg4(const void *p, long long i, T out[4]);
-template <>
-__device__ __forceinline__ void ldg4<float>(const void *p, long long i, float out[4]) {
-    const uint4 a = __ldcs(reinterpret_cast<const uint4 *>(static_cast<const float *>(p) + i));
-    out[0] = __uint_as_float(a.x), out[1] = __uint_as_float(a.y), out[2] = __uint_as_float(a.z), out[3] = __uint_as_float(a.w);
-}
-template <>
-__device__ __forceinline__ void ldg4<double>(const void *p, long long i, double out[4]) {
-    const uint4 *q = reinterpret_cast<const uint4 *>(static_cast<const double *>(p) + i);
-    const uint4 a = __ldcs(q), b = __ldcs(q + 1);
-    out[0] = __longlong_as_double(((long long)a.y << 32) | a.x), out[1] = __longlong_as_double(((long long)a.w << 32) | a.z);
-    out[2] = __longlong_as_double(((long long)b.y << 32) | b.x), out[3] = __longlong_as_double(((long long)b.w << 32) | b.z);
-}
 
 // CLAMPED index for fp32 keys: halves the load on the conversion pipe (F2F.F64.F32 + F2I.F64 per key on the quarter-rate XU
 // pipe).  The cell is a monotone function of the key (every step of
@@ -180,14 +154,15 @@ __device__ __forceinline__ unsigned group_rows_tail(const RingParams &p, long lo
 // A ring holds < 64 entries left over from the last flush + the new ones of one group; a flush moves whole LINES of 64 entries
 // (128 bytes).  With <= 32 new entries per part and group the ring never fills (the busiest part of the headline workload takes
 // 19 +- 4 of a group's 256 rows); rows that find it full go to direct REDs.
-template <typename T, int ND, int PPL, int FG>
+constexpr int kRing = 96;
+constexpr int kRingStride = kRing + 8; // 208 bytes: 16-byte aligned rows that rotate over the banks
+template <int PPL>
 struct RingLayout {
-    static constexpr int kRing = kLine == 64 ? 96 : 64;
-    static constexpr int kRingStride = kRing + 8; // 208 bytes: 16-byte aligned rows that rotate over the banks
-    static constexpr size_t kColBytes = 0; // the keys travel through registers
     static constexpr size_t kRingBytes = 32ull * PPL * kRingStride * 2;
     static constexpr size_t kCntBytes = 32ull * PPL * 4 + 256; // + the flush's (write position, owner) map
-    static constexpr size_t kPerWarp = kColBytes + kRingBytes + kCntBytes;
+    static constexpr size_t kPerWarp = kRingBytes + kCntBytes;
+    // two CTAs per SM; 24 warps per SM leave 85 registers per thread: the two key sets + the placement fit without spills
+    static constexpr int kWarps = std::min<int>(12, (113 * 1024 - 512) / kPerWarp);
 };
 
 // state of the parts a lane owns (parts lane, lane+32, ...): where the next granule goes
@@ -199,17 +174,17 @@ struct Owner {
     unsigned total[PPL]; // entries written to this list so far
 };
 
-template <typename T, int ND, int PPL, int FG, int WARPS, bool CLAMPED>
+template <typename T, int ND, int PPL, int WARPS, bool CLAMPED>
 __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_constant__ RingParams p) {
-    using L = RingLayout<T, ND, PPL, FG>;
-    constexpr int RING = L::kRing, RSTRIDE = L::kRingStride;
+    using L = RingLayout<PPL>;
+    constexpr int RING = kRing, RSTRIDE = kRingStride;
     static_assert(RING - kLine <= kLine && (RSTRIDE * 2) % 16 == 0, "ring geometry");
     extern __shared__ __align__(128) unsigned char dyn_smem[];
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned char *mine = dyn_smem + (size_t)warp * L::kPerWarp;
-    unsigned short *const ring = reinterpret_cast<unsigned short *>(mine + L::kColBytes); // [32*PPL][RING + 8]
-    unsigned *const cnt = reinterpret_cast<unsigned *>(mine + L::kColBytes + L::kRingBytes);
+    unsigned short *const ring = reinterpret_cast<unsigned short *>(mine); // [32*PPL][RING + 8]
+    unsigned *const cnt = reinterpret_cast<unsigned *>(mine + L::kRingBytes);
     uint2 *const fmap = reinterpret_cast<uint2 *>(cnt + 32 * PPL); // [32] {pool entry index, owner lane} of the lines of one flush
 #pragma unroll
     for (int k = 0; k < PPL; k++)
@@ -319,9 +294,8 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
     };
 
     // ---- complete groups of 256 rows: the keys of the NEXT group are loaded into registers (128-bit, evict-first) while the
-    // current one is placed: two register sets, the loop is unrolled by two so that no copy is needed.  (A TMA-staged variant
-    // spends instructions on issuing the bulk copies and waiting on the mbarriers, and 4 KB of shared memory per warp on the double
-    // buffer.)
+    // current one is placed: two register sets, the loop is unrolled by two so that no copy is needed.  (Staging them through shared
+    // memory instead would add shared-memory traffic to a kernel bound by the shared-memory pipe.)
     const long long ngroups = p.nrows / kGroupRows;
     auto load = [&](long long g, T (&dst)[2][ND][4]) {
         const long long r0 = p.row0 + g * kGroupRows + lane * 4;
@@ -329,7 +303,7 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
         for (int q = 0; q < 2; q++)
 #pragma unroll
             for (int d = 0; d < ND; d++)
-                ldg4<T>(p.x[d], r0 + q * 128, dst[q][d]);
+                ldcs4<T>(p.x[d], r0 + q * 128, dst[q][d]);
     };
     auto place = [&](const T (&c)[2][ND][4]) {
         unsigned idx[8], slots[8];
@@ -386,7 +360,7 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
 // entries, assuming the entries of a part are spread evenly over its warps (they are: the warps take row tiles round-robin).
 __global__ void __launch_bounds__(kCountThreads, 1) k_ring_count(const __grid_constant__ RingParams p) {
     extern __shared__ __align__(16) unsigned hist[];
-    __shared__ unsigned long long s_part_entries[kMaxParts + 1]; // exclusive prefix over parts
+    __shared__ unsigned long long s_part_entries[kRingParts + 1]; // exclusive prefix over parts
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nparts = p.nparts, npad = p.nparts_pad;
     const unsigned W = p.nlists_w;
@@ -469,46 +443,28 @@ __global__ void __launch_bounds__(kCountThreads, 1) k_ring_count(const __grid_co
     }
 }
 
-template <typename T, int ND, int PPL, int FG>
-int launch_partition_cfg(int sm_count, cudaStream_t st, RingParams &p, int *warps_out, bool dry, bool clamped) {
-    using L = RingLayout<T, ND, PPL, FG>;
-    constexpr int fit = (int)((113 * 1024 - 512) / L::kPerWarp); // two CTAs per SM
-    constexpr int WARPS = fit > 12 ? 12 : fit; // 24 warps per SM leave 85 registers per thread: the two key sets + the placement fit without spills
-    if constexpr (WARPS >= 2) {
-        const long long ngroups = (p.nrows + kGroupRows - 1) / kGroupRows;
-        // at least ~8 groups per warp so that the per-(warp, part) partial chunks stay a small share of the scratch
-        long long blocks = std::min<long long>((ngroups / 8 + WARPS - 1) / WARPS, (long long)sm_count * 2);
-        if (blocks < 1)
-            blocks = 1;
-        *warps_out = (int)blocks * WARPS;
-        if (dry)
+// CTAs of k_ring_partition for `nrows` rows: at least ~8 groups per warp so that the per-(warp, part) partial chunks stay a small
+// share of the scratch, at most two per SM
+long long partition_ctas(long long nrows, int warps, int sm_count) {
+    const long long ngroups = (nrows + kGroupRows - 1) / kGroupRows;
+    return std::max(std::min<long long>((ngroups / 8 + warps - 1) / warps, (long long)sm_count * 2), 1ll);
+}
+
+int launch_partition(const FloatPlan &f, bool clamped, long long ctas, cudaStream_t st, const RingParams &p) {
+    return with_keys(f, [&](auto t, auto nd) {
+        using T = decltype(t);
+        constexpr int ND = decltype(nd)::value;
+        auto go = [&](auto ppl) -> int {
+            constexpr int PPL = decltype(ppl)::value, WARPS = RingLayout<PPL>::kWarps;
+            auto kern = clamped ? k_ring_partition<T, ND, PPL, WARPS, std::is_same<T, float>::value> : k_ring_partition<T, ND, PPL, WARPS, false>;
+            constexpr size_t dyn = RingLayout<PPL>::kPerWarp * WARPS;
+            B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+            kern<<<(int)ctas, WARPS * 32, dyn, st>>>(p);
+            B200_CUDA(cudaGetLastError());
             return B200_OK;
-        auto kern = clamped ? k_ring_partition<T, ND, PPL, FG, WARPS, std::is_same<T, float>::value> : k_ring_partition<T, ND, PPL, FG, WARPS, false>;
-        constexpr size_t dyn = L::kPerWarp * WARPS;
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-        kern<<<(int)blocks, WARPS * 32, dyn, st>>>(p);
-        B200_CUDA(cudaGetLastError());
-        return B200_OK;
-    } else {
-        *warps_out = 0;
-        return B200_OK;
-    }
-}
-
-template <typename T, int ND>
-int launch_partition_nd(int sm_count, cudaStream_t st, RingParams &p, int *warps_out, bool dry, bool clamped) {
-    if (p.nparts_pad == 32)
-        return launch_partition_cfg<T, ND, 1, 1>(sm_count, st, p, warps_out, dry, clamped);
-    return launch_partition_cfg<T, ND, 2, 1>(sm_count, st, p, warps_out, dry, clamped);
-}
-
-template <typename T>
-int launch_partition(int nd, int sm_count, cudaStream_t st, RingParams &p, int *warps_out, bool dry, bool clamped) {
-    switch (nd) {
-    case 1: return launch_partition_nd<T, 1>(sm_count, st, p, warps_out, dry, clamped);
-    case 2: return launch_partition_nd<T, 2>(sm_count, st, p, warps_out, dry, clamped);
-    default: return launch_partition_nd<T, 3>(sm_count, st, p, warps_out, dry, clamped);
-    }
+        };
+        return p.nparts_pad == 32 ? go(std::integral_constant<int, 1>()) : go(std::integral_constant<int, 2>());
+    });
 }
 
 // ---- host side of the CLAMPED index (see bin_cell_m2_clamped) ---------------------------------------------------------------
@@ -586,44 +542,24 @@ bool magic_exact(unsigned cells, unsigned tile_cells, unsigned magic) {
 } // namespace
 
 // Scratch (pool + list tables) lives in the slot; grown on demand.
-int try_launch_ringcount(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool vec, bool *taken) {
+int launch_ringcount(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken) {
     *taken = false;
-    static const bool disabled = getenv("B200_DISABLE_RINGCOUNT") && atoi(getenv("B200_DISABLE_RINGCOUNT")) != 0;
-    static const bool no_clamp = getenv("B200_RING_NO_CLAMP") && atoi(getenv("B200_RING_NO_CLAMP")) != 0; // A/B knob
-    if (disabled || !vec || bp.nb < 1 || bp.nb > 3 || bp.na != 1 || bp.nrows < (1ll << 22))
-        return B200_OK;
-    const DevAgg &a = bp.a[0];
-    if (a.op != B200_AGG_COUNT || a.data || a.mask)
-        return B200_OK;
-    const unsigned long long cells = bp.cells;
-    if (cells * 4 <= 96 * 1024 || cells > (unsigned long long)kMaxTileCells * kMaxParts || cells >= (1ull << 22))
-        return B200_OK; // small grids: shared-memory privatisation; huge grids: direct REDs / region sort
-    const int t = bp.b[0].dtype;
-    if (t != B200_F32 && t != B200_F64)
-        return B200_OK;
+    const long long nrows = f.p.nrows;
+    const unsigned long long cells = f.p.cells;
     RingParams p;
     memset(&p, 0, sizeof p);
-    for (int i = 0; i < bp.nb; i++) {
-        const DevBinner &b = bp.b[i];
-        if (b.kind != B200_BINNER_SCALAR || b.dtype != t || b.byteswap || b.mask || b.bins < 1 || b.bins >= (1ull << 30))
-            return B200_OK;
-        p.x[i] = b.data;
-        p.vmin[i] = b.vmin;
-        p.scale[i] = b.scale;
-        p.bins_d[i] = b.bins_d;
-        p.bins[i] = (unsigned)b.bins;
-        p.stride[i] = (unsigned)b.stride;
-        p.stride_sum += (unsigned)b.stride;
-    }
-    bool clamped = t == B200_F32 && !no_clamp;
-    for (int i = 0; i < bp.nb && clamped; i++)
+    static_cast<FloatKeys &>(p) = f.p;
+    for (int i = 0; i < f.nd; i++)
+        p.stride_sum += p.stride[i];
+    bool clamped = f.xdtype == B200_F32;
+    for (int i = 0; i < f.nd && clamped; i++)
         clamped = clamp_bounds(p.vmin[i], p.scale[i], p.bins_d[i], p.bins[i], &p.clamp_lo[i], &p.clamp_hi[i]);
-    // as few parts as possible (32, else 64, else 128): the ring memory of k_ring_partition scales with the parts per lane;
+    // as few parts as possible (32, else 64): the ring memory of k_ring_partition scales with the parts per lane;
     // tile_cells is nudged upwards until the one-instruction division is exact
     unsigned tile_cells = 0, magic = 0;
-    for (int np = 32; np <= kMaxParts && !tile_cells; np *= 2) {
+    for (int np = 32; np <= kRingParts && !tile_cells; np *= 2) {
         unsigned long long tcells = ((cells + np - 1) / np + 7) / 8 * 8;
-        for (int tries = 0; tries < 64 && tcells <= kMaxTileCells; tries++, tcells += 8) {
+        for (int tries = 0; tries < 64 && tcells <= kRingTileCells; tries++, tcells += 8) {
             const unsigned m = (unsigned)((1ull << 32) / tcells) + 1u;
             if (magic_exact((unsigned)cells, (unsigned)tcells, m)) {
                 tile_cells = (unsigned)tcells;
@@ -640,21 +576,14 @@ int try_launch_ringcount(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool ve
     p.magic = magic;
     p.nparts = (int)((cells + tile_cells - 1) / tile_cells);
     p.nparts_pad = p.nparts <= 32 ? 32 : 64;
-    p.grid = static_cast<unsigned long long *>(a.grid);
+    p.grid = f.p.count_star;
 
     // batches of <= 2^30 rows (32-bit entry counts), EQUAL in size: a 2^30 + remainder split paid the fixed cost of a pass (memsets,
     // one histogram flush per SM and part) for a small second batch
-    const long long nbatch = (bp.nrows + (1ll << 30) - 1) >> 30;
-    const long long batch = std::min<long long>(bp.nrows, (((bp.nrows + nbatch - 1) / nbatch) + 255) & ~255ll);
-    p.row0 = 0;
-    p.nrows = batch;
-    int nwarps = 0;
-    if (t == B200_F32)
-        B200_CHECK(launch_partition<float>(bp.nb, ctx->sm_count, nullptr, p, &nwarps, true, clamped));
-    else
-        B200_CHECK(launch_partition<double>(bp.nb, ctx->sm_count, nullptr, p, &nwarps, true, false));
-    if (nwarps <= 0)
-        return B200_OK;
+    const long long nbatch = (nrows + (1ll << 30) - 1) >> 30;
+    const long long batch = std::min<long long>(nrows, (((nrows + nbatch - 1) / nbatch) + 255) & ~255ll);
+    const int warps = p.nparts_pad == 32 ? RingLayout<1>::kWarps : RingLayout<2>::kWarps; // per CTA of k_ring_partition
+    const long long nwarps = partition_ctas(batch, warps, ctx->sm_count) * warps;
     // chunk size: about a quarter of a (warp, part) list, within 512..2048 entries
     unsigned cshift = 9;
     while (cshift < 11 && (unsigned long long)batch / ((unsigned long long)nwarps * p.nparts) >= (8ull << cshift))
@@ -670,21 +599,11 @@ int try_launch_ringcount(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool ve
     // layout: [ctl 256 B | len | unused] (zeroed)  [head | next] (0xFF)  [pool]
     const size_t off_len = 256, off_unused = align_up(off_len + lists * 4, 256), zero_end = align_up(off_unused + nchunks * 2, 256);
     const size_t off_head = zero_end, off_next = align_up(off_head + lists * 4, 256), ff_end = align_up(off_next + nchunks * 4, 256);
-    const size_t off_pool = ff_end, need = off_pool + (nchunks << cshift) * 2;
-    if (slot->scratch_cap < need) {
-        if (slot->scratch) {
-            B200_CUDA(cudaStreamSynchronize(slot->stream));
-            B200_CUDA(cudaFree(slot->scratch));
-            slot->scratch = nullptr;
-            slot->scratch_cap = 0;
-        }
-        cudaError_t e = cudaMalloc(&slot->scratch, need);
-        if (e != cudaSuccess) { // not enough memory for the pool: the direct RED kernel takes the call
-            cudaGetLastError();
-            return B200_OK;
-        }
-        slot->scratch_cap = need;
-    }
+    const size_t off_pool = ff_end;
+    bool room = false;
+    B200_CHECK(slot_scratch(slot, off_pool + (nchunks << cshift) * 2, &room));
+    if (!room) // not enough memory for the pool: the direct RED kernel takes the call
+        return B200_OK;
     char *base = static_cast<char *>(slot->scratch);
     p.ctl = reinterpret_cast<unsigned *>(base);
     p.len = reinterpret_cast<unsigned *>(base + off_len);
@@ -693,18 +612,16 @@ int try_launch_ringcount(b200_ctx *ctx, Slot *slot, const BinParams &bp, bool ve
     p.next = reinterpret_cast<unsigned *>(base + off_next);
     p.pool = reinterpret_cast<unsigned short *>(base + off_pool);
     cudaStream_t st = slot->stream;
-    B200_CUDA(cudaFuncSetAttribute(k_ring_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((kMaxTileCells + 1) * 4)));
+    B200_CUDA(cudaFuncSetAttribute(k_ring_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((kRingTileCells + 1) * 4)));
     const size_t hist_bytes = ((size_t)tile_cells / 4 + 1) * 16;
-    for (long long r0 = 0; r0 < bp.nrows; r0 += batch) {
+    for (long long r0 = 0; r0 < nrows; r0 += batch) {
         p.row0 = r0;
-        p.nrows = std::min<long long>(batch, bp.nrows - r0);
+        p.nrows = std::min<long long>(batch, nrows - r0);
         B200_CUDA(cudaMemsetAsync(base, 0, zero_end, st));
         B200_CUDA(cudaMemsetAsync(base + off_head, 0xFF, ff_end - off_head, st));
-        int w = 0;
-        if (t == B200_F32)
-            B200_CHECK(launch_partition<float>(bp.nb, ctx->sm_count, st, p, &w, false, clamped));
-        else
-            B200_CHECK(launch_partition<double>(bp.nb, ctx->sm_count, st, p, &w, false, false));
+        const long long ctas = partition_ctas(p.nrows, warps, ctx->sm_count);
+        B200_CHECK(launch_partition(f, clamped, ctas, st, p));
+        const long long w = ctas * warps;
         p.nlists_w = (unsigned)w; // the last batch may launch fewer warps; its lists are the first w rows of head[] / len[]
         k_ring_count<<<ctx->sm_count, kCountThreads, hist_bytes, st>>>(p);
         B200_CUDA(cudaGetLastError());

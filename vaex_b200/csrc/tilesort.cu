@@ -12,8 +12,6 @@
 // Results are identical to fast.cu / the generic kernel for the counts; fp sums differ only by atomic ordering (as they do
 // between any two runs of those kernels).  Reference semantics: src/binners.cpp:13-57 (index), src/agg_count.cpp:53-57,
 // src/agg_sum.cpp:98-127 (NaN values skipped).
-#include <stdlib.h>
-
 #include <algorithm>
 
 #include "binby.cuh"
@@ -45,21 +43,17 @@ constexpr unsigned kPadIdx = 0xFFFFFFFFu;
 constexpr int kSlice = 2048;            // bucket entries per k_sort_apply CTA: small, so that the CTAs resident at any moment
                                         // (132 x 8) span only a few regions and their cells stay in the L2
 
-
+// 4 rows of a float / double column, widened to double
 template <typename T>
 __device__ __forceinline__ void load4(const void *p, long long i, double out[4]);
 template <>
 __device__ __forceinline__ void load4<float>(const void *p, long long i, double out[4]) {
-    uint4 a = __ldcs(reinterpret_cast<const uint4 *>(static_cast<const float *>(p) + i));
-    out[0] = (double)__uint_as_float(a.x), out[1] = (double)__uint_as_float(a.y), out[2] = (double)__uint_as_float(a.z), out[3] = (double)__uint_as_float(a.w);
+    float a[4];
+    ldcs4<float>(p, i, a);
+    out[0] = (double)a[0], out[1] = (double)a[1], out[2] = (double)a[2], out[3] = (double)a[3];
 }
 template <>
-__device__ __forceinline__ void load4<double>(const void *p, long long i, double out[4]) {
-    const uint4 *q = reinterpret_cast<const uint4 *>(static_cast<const double *>(p) + i);
-    uint4 a = __ldcs(q), b = __ldcs(q + 1);
-    out[0] = __longlong_as_double(((long long)a.y << 32) | a.x), out[1] = __longlong_as_double(((long long)a.w << 32) | a.z);
-    out[2] = __longlong_as_double(((long long)b.y << 32) | b.x), out[3] = __longlong_as_double(((long long)b.w << 32) | b.z);
-}
+__device__ __forceinline__ void load4<double>(const void *p, long long i, double out[4]) { ldcs4<double>(p, i, out); }
 
 __device__ __forceinline__ void l2_prefetch(const void *p, unsigned bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
@@ -306,55 +300,34 @@ __global__ void __launch_bounds__(256) k_sort_apply(const __grid_constant__ Sort
             apply_row<HASV>(p.f, idx[k], HASV ? val[k] : 0.0);
 }
 
-template <typename T, int ND, typename TV, bool HASV>
-int launch_partition(int sm_count, cudaStream_t st, const SortParams &p) {
-    constexpr size_t dyn = warp_bytes<HASV>() * kWarps;
+int launch_partition(const FloatPlan &f, int sm_count, cudaStream_t st, const SortParams &p) {
     const long long ntiles = (p.nrows + kWarpTile * kWarps - 1) / (kWarpTile * kWarps);
     const int blocks = (int)std::min<long long>(ntiles, (long long)sm_count * 2);
-#define B200_SORT_LAUNCH(PPL)                                                                                   \
-    do {                                                                                                         \
-        auto kern = k_sort_partition<T, ND, TV, HASV, PPL>;                                                      \
-        B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));           \
-        kern<<<blocks, kWarps * 32, dyn, st>>>(p);                                                               \
-    } while (0)
-    if (p.nparts <= 64) // (the region count is 33..64 by construction, up to 128 when a region would exceed its byte budget)
-        B200_SORT_LAUNCH(2);
-    else
-        B200_SORT_LAUNCH(4);
-#undef B200_SORT_LAUNCH
-    B200_CUDA(cudaGetLastError());
-    return B200_OK;
-}
-
-template <typename T, int ND>
-int launch_partition_v(int sm_count, cudaStream_t st, const SortParams &p, int vdtype) {
-    if (!p.f.v)
-        return launch_partition<T, ND, double, false>(sm_count, st, p);
-    if (vdtype == B200_F32)
-        return launch_partition<T, ND, float, true>(sm_count, st, p);
-    return launch_partition<T, ND, double, true>(sm_count, st, p);
-}
-
-template <typename T>
-int launch_partition_nd(int nd, int sm_count, cudaStream_t st, const SortParams &p, int vdtype) {
-    switch (nd) {
-    case 1: return launch_partition_v<T, 1>(sm_count, st, p, vdtype);
-    case 2: return launch_partition_v<T, 2>(sm_count, st, p, vdtype);
-    default: return launch_partition_v<T, 3>(sm_count, st, p, vdtype);
-    }
+    return with_keys(f, [&](auto t, auto nd) {
+        using T = decltype(t);
+        constexpr int ND = decltype(nd)::value;
+        auto go = [&](auto tv, auto hasv) -> int {
+            using TV = decltype(tv);
+            constexpr bool HASV = decltype(hasv)::value;
+            constexpr size_t dyn = warp_bytes<HASV>() * kWarps;
+            // (the region count is 33..64 by construction, up to 128 when a region would exceed its byte budget)
+            auto kern = p.nparts <= 64 ? k_sort_partition<T, ND, TV, HASV, 2> : k_sort_partition<T, ND, TV, HASV, 4>;
+            B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+            kern<<<blocks, kWarps * 32, dyn, st>>>(p);
+            B200_CUDA(cudaGetLastError());
+            return B200_OK;
+        };
+        if (!p.f.v)
+            return go(double(), std::false_type());
+        return f.vdtype == B200_F32 ? go(float(), std::true_type()) : go(double(), std::true_type());
+    });
 }
 
 } // namespace
 
-int try_launch_tilesort(b200_ctx *ctx, Slot *slot, const FastParams &fp, int xdtype, int nd, int vdtype, bool *taken) {
+int launch_tilesort(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken) {
     *taken = false;
-    // tuning knobs, read per call (tests shrink them to reach every variant with small inputs)
-    auto env_ll = [](const char *name, long long dflt) {
-        const char *e = getenv(name);
-        return e && *e ? atoll(e) : dflt;
-    };
-    if (env_ll("B200_DISABLE_TILESORT", 0) || fp.nrows < env_ll("B200_TILESORT_MIN_ROWS", 1ll << 24) || fp.smem_copies)
-        return B200_OK;
+    const FastParams &fp = f.p;
     const unsigned long long region_bytes = (unsigned long long)env_ll("B200_TILESORT_REGION_KB", 16 << 10) << 10;
     const int naggs = (fp.count_star != nullptr) + (fp.vcount != nullptr) + (fp.vsum != nullptr) + (fp.vm2 != nullptr);
     const unsigned long long cells = fp.cells;
@@ -375,20 +348,10 @@ int try_launch_tilesort(b200_ctx *ctx, Slot *slot, const FastParams &fp, int xdt
     const long long batch = std::min<long long>(fp.nrows, 1ll << 27);
     const unsigned long long cap = (((unsigned long long)batch * 4 / nparts + 65536) + kChunk - 1) / kChunk * kChunk;
     const size_t entry = 4 + (fp.v ? 8 : 0);
-    const size_t need = 4096 + (size_t)nparts * cap * entry;
-    if (slot->scratch_cap < need) {
-        if (slot->scratch) {
-            B200_CUDA(cudaStreamSynchronize(slot->stream));
-            B200_CUDA(cudaFree(slot->scratch));
-            slot->scratch = nullptr;
-            slot->scratch_cap = 0;
-        }
-        if (cudaMalloc(&slot->scratch, need) != cudaSuccess) { // no room for the buckets: the caller scatters directly
-            cudaGetLastError();
-            return B200_OK;
-        }
-        slot->scratch_cap = need;
-    }
+    bool room = false;
+    B200_CHECK(slot_scratch(slot, 4096 + (size_t)nparts * cap * entry, &room));
+    if (!room) // no room for the buckets: the caller scatters directly
+        return B200_OK;
     char *base = static_cast<char *>(slot->scratch);
     p.cursors = reinterpret_cast<unsigned *>(base);
     p.bval = reinterpret_cast<double *>(base + 4096); // the 8-byte entries first (alignment)
@@ -400,10 +363,7 @@ int try_launch_tilesort(b200_ctx *ctx, Slot *slot, const FastParams &fp, int xdt
         p.row0 = r0;
         p.nrows = std::min<long long>(batch, fp.nrows - r0);
         B200_CUDA(cudaMemsetAsync(p.cursors, 0, 4096, st));
-        if (xdtype == B200_F32)
-            B200_CHECK(launch_partition_nd<float>(nd, ctx->sm_count, st, p, vdtype));
-        else
-            B200_CHECK(launch_partition_nd<double>(nd, ctx->sm_count, st, p, vdtype));
+        B200_CHECK(launch_partition(f, ctx->sm_count, st, p));
         const long long ctas = (long long)nparts * nslices;
         if (fp.v)
             k_sort_apply<true><<<(unsigned)ctas, 256, 0, st>>>(p, nslices);
