@@ -31,6 +31,8 @@
  *                         isin / create-from-keys, and hash<T> (src/hash.hpp:40-152).
  *   b200_minmax           the limits pre-pass: vaexfast statisticNd OP_MIN_MAX (src/vaexfast.cpp:1089-1101).
  *   b200_stat_*           TaskPartStatistic + vaexfast statisticNd_f4/_f8, every op (vaex/cpu.py:487-626, src/vaexfast.cpp:1061-1278).
+ *   b200_grid_percentile  the finish of percentile_approx (vaex/dataframe.py:1675-1754) with vaexfast.grid_find_edges
+ *                         (src/vaexfast.cpp:1680-1719), on a device count grid.
  *   b200_hash64           superutils.hash (src/superutils.cpp:265) — test hook, host only.
  */
 #ifndef B200AGG_H
@@ -271,6 +273,21 @@ int b200_stat_fields(const b200_stat *stat);
 int b200_stat_read(b200_stat *stat, double *out);
 int b200_stat_reset(b200_stat *stat);
 int b200_stat_destroy(b200_stat *stat);
+
+/* ---- percentile_approx / median_approx: the finish of a count grid (vaex/dataframe.py:1675-1754) ----------------------------
+ * `grid` is a DEVICE int64 count grid with edges, first dimension fastest: the binby dimensions, then the percentile axis last,
+ * `sizes` = its ndim sizes including the +3 of edges (b200_agg_device_ptr of a count(*) aggregator, a grid after an all-reduce, or
+ * any grid built by the caller).  Binby axes are sliced [2:-1], the percentile axis [1:] (:1679-1683).  For each percentage pct[k]
+ * (not 0 or 100, which the caller returns as the limits themselves, :1699-1704) out[k * cells + cell] receives the interpolated
+ * percentile of that sliced binby cell, cells first binner fastest: the int64 cumulative sum, the targets floor / ceil of
+ * (total + 1) * pct / 100. (an int64 product first when integral[k] != 0, as numpy evaluates an integer percentage; 0 for an empty
+ * cell), vaexfast.grid_find_edges (src/vaexfast.cpp:1680-1719) and calculate_x (:1725-1744) with `lb` and `span` = ub - lb as the
+ * caller's numpy evaluated it in the limits' dtype.  With two or more binby dimensions every cell gets what the reference's
+ * one-dimensional code gives for that cell; the reference's own search reads outside its grid there (:1694-1698).
+ * `out` is host memory (memspace_out = B200_MEM_HOST) or device memory (B200_MEM_DEVICE); the call waits for the result.
+ * ndim <= B200_MAX_BINNERS. */
+int b200_grid_percentile(b200_ctx *ctx, int slot, const int64_t *grid, int ndim, const int64_t *sizes, double lb, double span, const double *pct,
+                         const uint8_t *integral, int npct, int memspace_out, double *out);
 
 /* ---- device-side expressions and filter compaction (SURVEY.md section 8f row 2) ------------------------------------------------
  * Replaces the per-chunk Python `eval` of virtual columns / filters / selections (vaex/scopes.py:108-128 _BlockScope.evaluate) and

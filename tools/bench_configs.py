@@ -2,7 +2,7 @@
 """Times every BASELINE.json configuration on one H100 with device-resident columns (the roofline setting) and prints one
 JSON object per config: rows/s, achieved algorithmic GB/s (SURVEY.md 8d bytes/row) and the fraction of the measured HBM peak.
 
-    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV]
+    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV,PA]
 
 This is a companion to bench.py (which owns the headline line the driver parses); results are quoted in DESIGN.md.
 """
@@ -233,6 +233,60 @@ def main():
             del k1, k2, v
         elif cfg == "LS":
             ls_string_list(args, ctx, stream, gen, report)
+        elif cfg == "PA":
+            pa_percentile(args, n, ctx, stream, gen, timed, report)
+
+
+def pa_percentile(args, n, ctx, stream, gen, timed, report):
+    """PA: df.percentile_approx(z, [25, 50, 75]) over `n` device-resident fp32 rows, (a) binby=[x, y] 128^2 in [-3, 3] with 1024
+    percentile bins in [-4, 4] (a 131^2 x 1027 int64 grid, 141 MB: k_pct_cell) and (b) no binby with 65536 percentile bins (one cell:
+    k_pct_block).  Timed separately with CUDA events: the count pass and the device finish (b200_grid_percentile).  Beside them the host
+    finish the reference runs: the D2H of the count grid into pageable memory and the vectorised numpy restatement of the finish
+    (tests/percentile_oracle.py), which is a lower bound of the reference's own, whose index_choose loops over every cell in Python."""
+    import subprocess
+    import numpy as np
+    import torch
+    from vaex_b200 import percentile as _pct, superagg
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import percentile_oracle as PO
+    power = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    cols = [torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen) for _ in range(3)]
+    pct = [25, 50, 75]
+    for name, nd, P in (("PA-2d", 2, 1024), ("PA-none", 0, 65536)):
+        bs = [superagg.BinnerScalar_float32(1, "xy"[i], -3.0, 3.0, 128) for i in range(nd)] + [superagg.BinnerScalar_float32(1, "z", -4.0, 4.0, P)]
+        g = superagg.Grid(bs)
+        for b, c in zip(bs, cols[2 - nd:]):
+            b.set_data(0, c)
+        a = superagg.AggCount_int64(g, 1, 1)
+
+        def count():
+            a.reset(0)
+            g.bin(0, [a], n)
+        ms_count = timed(count, args.reps)
+        ptr, nbytes = a.device_pointer(0)
+        cells = int(np.prod([s - 3 for s in g.shapes[:-1]], dtype=np.int64))
+        out = torch.empty((len(pct), cells), dtype=torch.float64, device="cuda")
+        ms_finish = timed(lambda: _pct.grid_percentile(ptr, g.shapes, -4.0, 8.0, pct, ctx=ctx, out=out), args.reps)
+        host_best = d2h_best = None
+        for _ in range(max(2, args.reps // 2)):
+            t0 = time.perf_counter()
+            grid = a.get_result()  # D2H into pageable memory
+            t1 = time.perf_counter()
+            want = PO.percentile_approx([grid], [[-4, 4]], pct, False)
+            t2 = time.perf_counter()
+            d2h_best = min(d2h_best or 1e30, (t1 - t0) * 1e3)
+            host_best = min(host_best or 1e30, (t2 - t0) * 1e3)
+        got = out.cpu().numpy().reshape((len(pct),) + tuple(s - 3 for s in g.shapes[:-1]), order="F")
+        assert int(grid.sum()) == n and np.array_equal(got.view(np.int64), np.asarray(want).reshape(got.shape).view(np.int64))
+        workload = "percentile_approx(z, [25, 50, 75]" + (", binby=[x, y] shape 128" if nd else "") + f", percentile_shape={P}) on fp32 rows"
+        report(name + "/count", workload + ": count pass", n, 4 * (nd + 1), ms_count, gpu=power)
+        print(json.dumps(dict(config=name + "/finish", workload=workload + ": finish on the device", kernel="k_pct_cell" if cells >= 2048 else "k_pct_block",
+                              ms=ms_finish, grid_bytes=nbytes, grid_reads_gbs=2 * nbytes / (ms_finish * 1e-3) / 1e9, gpu=power)), flush=True)
+        print(json.dumps(dict(config=name + "/host_finish", workload=workload + ": D2H (pageable) + numpy finish on the host", ms=host_best, d2h_ms=d2h_best,
+                              grid_bytes=nbytes, gpu=power)), flush=True)
+        del a, g, out, grid
+        torch.cuda.empty_cache()
+    del cols
 
 
 def ls_string_list(args, ctx, stream, gen, report):

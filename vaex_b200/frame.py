@@ -6,6 +6,9 @@ pre-pass, dataframe.py:1519-1521, 1926-1928) and ``df.groupby(by).agg({...})`` (
 Columns are plain arrays: numpy (host; streamed in chunks) or device arrays (torch CUDA tensors; one fused pass).
 Expressions are column NAMES only — the expression system is upstream of the path and out of scope.
 """
+import ast
+import re
+
 import numpy as np
 
 from . import _lib
@@ -269,10 +272,102 @@ class Frame:
         with np.errstate(invalid="ignore"):
             return res.astype(dt)
 
-    def limits(self, expressions, value="minmax"):
+    def limits(self, expressions, value="minmax", selection=None):
+        """df.limits (vaex/dataframe.py:1844-2004): the (min, max) pair `value` describes per expression: "minmax", "N%"
+        (limits_percentage) or an explicit pair, returned as given.  `value` may also hold one of those per expression."""
         if isinstance(expressions, str):
-            return self.minmax(expressions)
-        return np.array([self.minmax(e) for e in expressions])
+            return self._limit(expressions, value, selection)
+        return np.array(self._limits_list(expressions, value, selection))
+
+    def _limits_list(self, expressions, value, selection):
+        if value is None:
+            value = "minmax"
+        values = (value,) * len(expressions) if _is_limit(value) or not _issequence(value) else value
+        return [self._limit(e, v, selection) for e, v in zip(expressions, values)]
+
+    def _limit(self, expression, value, selection=None):
+        if _is_limit(value):
+            return value
+        if value is None or value == "minmax":
+            return self.minmax(expression, selection=selection)
+        match = re.match(r"([\d.]*)(\D*)", value)
+        number, kind = match.groups()
+        if kind.strip() in ("%", "percent"):
+            return self.limits_percentage(expression, ast.literal_eval(number), selection=selection)
+        raise NotImplementedError(f"limits {value!r}: only 'minmax', 'N%' and explicit [min, max] pairs are supported")
+
+    def limits_percentage(self, expression, percentage=99.73, square=False, selection=None):
+        """df.limits_percentage (vaex/dataframe.py:1795-1842): a range around the median holding about `percentage` % of the rows, read
+        off the normalised cumulative counts of a 16384-bin count between the minmax limits (np.interp on the host)"""
+        from . import percentile as _pct
+        waslist, expressions = _pct.listify(expression)
+        out = []
+        for e in expressions:
+            limits_minmax = self.minmax(e, selection=selection)
+            vmin, vmax = limits_minmax
+            size = 1024 * 16
+            counts = self.count(binby=e, shape=size, limits=limits_minmax, selection=selection)
+            cumcounts = np.concatenate([[0], np.cumsum(counts)])
+            cumcounts = cumcounts / cumcounts.max()
+            f = (1 - percentage / 100.) / 2
+            x = np.linspace(vmin, vmax, size + 1)
+            out.append(np.interp([f, 1 - f], cumcounts, x))
+        return _pct.unlistify(waslist, out)
+
+    # ---- approximate percentiles: one count pass, the finish on the device (csrc/percentile.cu) -----------------------------
+    def percentile_approx(self, expression, percentage=50., binby=None, limits=None, shape=128, percentile_shape=1024, percentile_limits="minmax",
+                          selection=None):
+        """df.percentile_approx (vaex/dataframe.py:1632-1780): the percentile(s) `percentage` of one expression or a list, optionally per
+        cell of a binby grid, interpolated in the cumulative counts of a `percentile_shape`-bin count between `percentile_limits` (one
+        pair or "minmax" / "N%" for all expressions, or one per expression).  Every expression's count grid is built in the same pass
+        and finished on the device.  With two or more binby dimensions each cell gets the answer of the reference's one-dimensional
+        code for that cell (DESIGN.md section 3)."""
+        from . import percentile as _pct
+        waslist, expressions = _pct.listify(expression)
+        expressions = [str(e) for e in expressions]
+        binby = [] if binby is None else ([binby] if not isinstance(binby, (list, tuple)) else list(binby))
+        selection = None if selection is False else selection
+        shape = _expand_shape(shape, len(binby))
+        percentile_shapes = _expand_shape(percentile_shape, len(expressions))
+        if percentile_limits:
+            percentile_limits = _expand_limits(percentile_limits, len(expressions))
+        f = self
+        missing = [e for e in expressions + binby if e not in self.columns]
+        if missing:
+            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
+            for e in missing:
+                f.columns[e] = f.expression(e)
+        for e in expressions + binby:
+            if e in f.categories or _dtype_of(f.columns[e]).kind in "mM":
+                raise NotImplementedError(f"percentile_approx over the categorical or datetime column {e!r} is not supported")
+        binby_limits = f._limits_list(binby, limits, selection)
+        expression_limits = f._limits_list(expressions, percentile_limits, selection)
+        mask = f.expression(selection) if isinstance(selection, str) else selection
+        if isinstance(selection, str) and mask.dtype != np.bool_:
+            raise ValueError("a selection must be a boolean expression")
+        dtypes = f.dtypes()
+        nthreads = f.executor.nthreads
+
+        def spec(e, count, lim):
+            return {"binner-type": "scalar", "expression": e, "dtype": dtypes[e].str, "count": int(count), "minimum": float(lim[0]),
+                    "maximum": float(lim[1])}
+        tasks = []
+        for e, pshape, plim in zip(expressions, percentile_shapes, expression_limits):
+            specs = [spec(b, n, lim) for b, n, lim in zip(binby, shape, binby_limits)] + [spec(e, pshape, plim)]
+            desc = _agg.count("*", selection=None if mask is None else "selection", edges=True)
+            desc._prepare_types(dtypes)
+            part = taskpart.TaskPartPercentile(None, [taskpart.decode_binner(s, nthreads) for s in specs], [desc], dtypes, plim, percentage,
+                                               nthreads=nthreads)
+            tasks.append(execution.Task(part, [mask]))
+        f.executor.execute(f.columns, tasks, f.length, filter=f._filter)
+        return _pct.unlistify(waslist, np.array([t.result for t in tasks]))
+
+    def median_approx(self, expression, percentage=50., binby=None, limits=None, shape=128, percentile_shape=256, percentile_limits="minmax",
+                      selection=None):
+        """df.median_approx (vaex/dataframe.py:1611-1629): percentile_approx at the integer percentage 50 (`percentage` is ignored, as
+        there), 256 percentile bins by default"""
+        return self.percentile_approx(expression, 50, binby=binby, limits=limits, shape=shape, percentile_shape=percentile_shape,
+                                      percentile_limits=percentile_limits, selection=selection)
 
     # ---- binned statistics -------------------------------------------------------------------------------------------
     def _binner_specs(self, binby, limits, shape):
@@ -608,6 +703,32 @@ class GroupBy:
             out[label] = _take_cells(g, flat) if _is_arrow(g) else g[center][keep]
         out["count"] = counts[keep]
         return out
+
+
+def _issequence(x):
+    return isinstance(x, (tuple, list, np.ndarray))
+
+
+def _is_limit(x):
+    """vaex.utils._is_limit: a sequence of numbers"""
+    import numbers
+    return _issequence(x) and all(isinstance(k, numbers.Number) for k in x)
+
+
+def _expand_shape(shape, dimension):
+    """vaex.utils._expand_shape"""
+    if isinstance(shape, (tuple, list)):
+        assert len(shape) == dimension, "wants to expand shape %r to dimension %d" % (shape, dimension)
+        return tuple(shape)
+    return (shape,) * dimension
+
+
+def _expand_limits(limits, dimension):
+    """vaex.utils._expand_limits"""
+    if _issequence(limits) and (_issequence(limits[0]) or isinstance(limits[0], str) or limits[0] is None):
+        assert len(limits) == dimension, "wants to expand shape %r to dimension %d" % (limits, dimension)
+        return tuple(limits)
+    return (limits,) * dimension
 
 
 def _is_arrow(x):

@@ -203,6 +203,29 @@ class TaskPartAggregation(TaskPart):
         return encoded
 
 
+class TaskPartPercentile(TaskPartAggregation):
+    """percentile_approx / median_approx of one expression (vaex/dataframe.py:1632-1780): the count(*) pass over binby + [expression]
+    with edges (:1668-1672) on one device grid, then the finish on that grid (csrc/percentile.cu).  Only the percentiles are read
+    back; the count grid never leaves the device.  ``limit`` is the expression's (lb, ub) pair as the limits pre-pass returned it."""
+    snake_name = "percentile_approx"
+
+    def __init__(self, df, binners, aggregation_descriptions, dtypes, limit, percentage, nthreads=None):
+        super().__init__(df, binners, aggregation_descriptions, dtypes, nthreads=nthreads)
+        (desc, selections, ops, _), = self.aggregations
+        if len(ops) != 1 or desc.expressions:
+            raise ValueError("a percentile task part holds one count(*) aggregator with one selection")
+        self.limit = limit
+        self.percentage = percentage
+
+    def get_result(self):
+        from . import percentile as _pct
+        op = self.aggregations[0][2][0]
+        if op.device_dtype != np.int64:
+            raise RuntimeError("the percentile finish reads an int64 count grid")
+        ptr, _ = op.device_pointer(0)
+        return _pct.finish(ptr, self.grid.shapes, self.limit, self.percentage, op._ctx)
+
+
 class RowLimitException(ValueError):
     pass
 
