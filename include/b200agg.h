@@ -305,7 +305,10 @@ typedef enum {
     B200_EX_CAST,   /* astype(b200_dtype arg) */
     B200_EX_ORDINAL /* _ordinal_values(value, sets[arg]) -> int64 ordinal, -1 when absent (vaex/functions.py:2454-2463) */
 } b200_expr_opcode;
-typedef enum { B200_EXC_F64 = 0, B200_EXC_F32, B200_EXC_I64 /* any signed integer, sign-extended */, B200_EXC_U64, B200_EXC_BOOL } b200_expr_class;
+/* I64_U64 / U64_I64: comparisons only, a signed integer (sign-extended) against a uint64, compared by exact value like numpy's
+   mixed-sign comparison loops; the name gives the operands' order */
+typedef enum { B200_EXC_F64 = 0, B200_EXC_F32, B200_EXC_I64 /* any signed integer, sign-extended */, B200_EXC_U64, B200_EXC_BOOL,
+               B200_EXC_I64_U64, B200_EXC_U64_I64 } b200_expr_class;
 typedef struct {
     int32_t op, cls, arg, reserved;
     double f;

@@ -135,6 +135,12 @@ __device__ __forceinline__ long long f64_to_i64_x86(double x) {
         return (long long)0x8000000000000000ULL;
     return __double2ll_rz(x);
 }
+// the 32-bit cvttsd2si (numpy's float -> int8/int16/int32/uint8/uint16 loops go through it): NaN / out of range -> INT32_MIN
+__device__ __forceinline__ int f64_to_i32_x86(double x) {
+    if (!(x == x) || x >= 2147483648.0 || x < -2147483648.0)
+        return (int)0x80000000u;
+    return __double2int_rz(x);
+}
 // gcc's x86-64 double -> uint64 sequence: below 2^63 cvttsd2si as above, else cvttsd2si(x - 2^63) ^ 2^63; so >= 2^64 -> 0
 __device__ __forceinline__ unsigned long long f64_to_u64_x86(double x) {
     if (x >= 9223372036854775808.0)

@@ -122,12 +122,20 @@ __device__ __forceinline__ Val cast_val(Val v, int from, int dtype) {
         case B200_EXC_F32: r.u = v.s != 0.f; break;
         default: r.u = v.u != 0; break;
         }
-    } else { // integers: C conversion of floats (x86 cvttsd2si for what does not fit), wrap for integers
-        switch (from) {
-        case B200_EXC_F64: r.i = f64_to_i64_x86(v.d); break;
-        case B200_EXC_F32: r.i = f64_to_i64_x86((double)v.s); break;
-        default: r.u = v.u; break;
-        }
+    } else if (from == B200_EXC_F64 || from == B200_EXC_F32) {
+        // floats: numpy's x86-64 casts.  int64 and uint32 take the 64-bit cvttsd2si (out of range / NaN -> INT64_MIN), then uint32
+        // wraps (numpy's scalar loop; its vector loop differs out of range, DESIGN §3); uint64 takes gcc's two-step sequence; the
+        // narrower types take the 32-bit cvttsd2si (out of range / NaN -> INT32_MIN), then wrap
+        const double x = from == B200_EXC_F64 ? v.d : (double)v.s;
+        if (dtype == B200_U64)
+            r.u = f64_to_u64_x86(x);
+        else if (dtype == B200_I64 || dtype == B200_U32)
+            r.i = f64_to_i64_x86(x);
+        else
+            r.i = f64_to_i32_x86(x);
+        r = wrap_int(r, dtype);
+    } else {
+        r.u = v.u;
         r = wrap_int(r, dtype);
     }
     return r;
@@ -270,6 +278,10 @@ __global__ void __launch_bounds__(256) k_eval(const __grid_constant__ EvalParams
                         lt = a.s < b.s, eq = a.s == b.s;
                     else if (c == B200_EXC_I64)
                         lt = a.i < b.i, eq = a.i == b.i;
+                    else if (c == B200_EXC_I64_U64) // a negative signed value is below every uint64
+                        lt = a.i < 0 || a.u < b.u, eq = a.i >= 0 && a.u == b.u;
+                    else if (c == B200_EXC_U64_I64)
+                        lt = b.i >= 0 && a.u < b.u, eq = b.i >= 0 && a.u == b.u;
                     else
                         lt = a.u < b.u, eq = a.u == b.u;
                     bool gt;

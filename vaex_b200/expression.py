@@ -20,7 +20,8 @@ from . import _lib
 
 (EX_INPUT, EX_CONST_F64, EX_CONST_I64, EX_ADD, EX_SUB, EX_MUL, EX_DIV, EX_NEG, EX_ABS, EX_SQRT, EX_LT, EX_LE, EX_GT, EX_GE, EX_EQ, EX_NE, EX_AND, EX_OR, EX_NOT,
  EX_CAST, EX_ORDINAL) = range(21)
-EXC_F64, EXC_F32, EXC_I64, EXC_U64, EXC_BOOL = range(5)
+# I64_U64 / U64_I64: comparisons of a signed integer with a uint64 by exact value, the operands in the order of the name
+EXC_F64, EXC_F32, EXC_I64, EXC_U64, EXC_BOOL, EXC_I64_U64, EXC_U64_I64 = range(7)
 
 _BINOPS = {ast.Add: (EX_ADD, np.add), ast.Sub: (EX_SUB, np.subtract), ast.Mult: (EX_MUL, np.multiply), ast.Div: (EX_DIV, np.true_divide)}
 _CMPOPS = {ast.Lt: EX_LT, ast.LtE: EX_LE, ast.Gt: EX_GT, ast.GtE: EX_GE, ast.Eq: EX_EQ, ast.NotEq: EX_NE}
@@ -39,6 +40,11 @@ def _cls(dtype):
     if dtype.kind == "u":
         return EXC_U64
     raise NotImplementedError(f"dtype {dtype} is not supported in device expressions")
+
+
+def _i64(v):
+    """an integer constant's 64-bit pattern as a signed int (uint64 values >= 2^63 wrap)"""
+    return v - (1 << 64) if v >= 1 << 63 else v
 
 
 class _Node:
@@ -80,13 +86,17 @@ class Program:
     def _materialise(self, node, dtype):
         """push-time resolution of a weak scalar: it becomes a constant of `dtype`"""
         dtype = np.dtype(dtype)
-        value = np.asarray(node.scalar).astype(dtype)[()]  # numpy's own conversion of the literal
+        if dtype.kind == "f" and isinstance(node.scalar, int):
+            # numpy converts a Python int to a double first (OverflowError beyond it), then to the float type: two roundings
+            value = np.float64(float(node.scalar)).astype(dtype)
+        else:
+            value = np.asarray(node.scalar).astype(dtype)[()]  # numpy's own conversion of the literal
         c = _cls(dtype)
         pos = node.slot
         if c in (EXC_F64, EXC_F32):
             self.ops[pos] = (EX_CONST_F64, c, 0, float(value), 0)
         else:
-            self.ops[pos] = (EX_CONST_I64, c, 0, 0.0, int(value))
+            self.ops[pos] = (EX_CONST_I64, c, 0, 0.0, _i64(int(value)))
         return _Node(dtype)
 
     def _cast(self, node, dtype):
@@ -146,18 +156,15 @@ class Program:
             b = self._emit(n.right)
             return self._binary(opcode, ufunc, a, b, mark)
         if isinstance(n, ast.Compare):
-            result = None
-            left = self._emit(n.left)
             if len(n.ops) != 1:
                 raise NotImplementedError("chained comparisons are not supported in device expressions (numpy rejects them too)")
-            mark = len(self.ops)
-            right = self._emit(n.comparators[0])
             if type(n.ops[0]) not in _CMPOPS:
                 raise NotImplementedError(type(n.ops[0]).__name__)
-            a, b, common = self._promote(left, right, mark, np.less)
-            self._op(_CMPOPS[type(n.ops[0])], _cls(common))
-            result = _Node(np.bool_)
-            return result
+            start = len(self.ops)
+            left = self._emit(n.left)
+            mark = len(self.ops)
+            right = self._emit(n.comparators[0])
+            return self._compare(_CMPOPS[type(n.ops[0])], left, right, start, mark)
         if isinstance(n, ast.Call):
             return self._call(n)
         if isinstance(n, ast.Attribute):
@@ -194,6 +201,40 @@ class Program:
             b = self._cast(b, common)
         return a, b, np.dtype(common)
 
+    def _compare(self, opcode, a, b, start, mark):
+        """a comparison; `start` / `mark` = index of the first op of a's / b's code"""
+        lit, col = (a, b) if a.weak else (b, a)
+        if lit.weak and not col.weak and col.dtype.kind in "iu" and isinstance(lit.scalar, int):
+            return self._compare_int_literal(opcode, a, b, start)
+        if not a.weak and not b.weak and {a.dtype.kind, b.dtype.kind} == {"i", "u"} and np.dtype(np.uint64) in (a.dtype, b.dtype):
+            # numpy compares a signed integer with a uint64 by exact value (its qQ / Qq loops), not through float64
+            self._op(opcode, EXC_I64_U64 if a.dtype.kind == "i" else EXC_U64_I64)
+            return _Node(np.bool_)
+        a, b, common = self._promote(a, b, mark, np.less)
+        self._op(opcode, _cls(common))
+        return _Node(np.bool_)
+
+    def _compare_int_literal(self, opcode, a, b, start):
+        """integer column against a Python int: numpy compares by the literal's value, whatever the column's width"""
+        lit, col = (a, b) if a.weak else (b, a)
+        v = lit.scalar
+        if v >= 1 << 64 or v < -(1 << 63):
+            # beyond every 64-bit value: the answer does not depend on the row, so the operand's code is dropped
+            less = (v > 0) == (b is lit)  # a < b on every row
+            result = {EX_LT: less, EX_LE: less, EX_GT: not less, EX_GE: not less, EX_EQ: False, EX_NE: True}[opcode]
+            del self.ops[start:]
+            self._op(EX_CONST_I64, EXC_BOOL, i=int(result))
+            return _Node(np.bool_)
+        col_signed = col.dtype.kind == "i"
+        lit_signed = col_signed if 0 <= v < 1 << 63 else v < 0
+        self.ops[lit.slot] = (EX_CONST_I64, EXC_I64 if lit_signed else EXC_U64, 0, 0.0, _i64(v))
+        if lit_signed == col_signed:
+            cls = EXC_I64 if col_signed else EXC_U64
+        else:
+            cls = EXC_I64_U64 if (col_signed if a is col else lit_signed) else EXC_U64_I64
+        self._op(opcode, cls)
+        return _Node(np.bool_)
+
     def _binary(self, opcode, ufunc, a, b, mark):
         a, b, common = self._promote(a, b, mark, ufunc)
         if common == np.bool_:
@@ -212,8 +253,8 @@ class Program:
             dt = np.dtype(n.args[0].value)
             if dt.name not in _lib.DTYPE_CODE:
                 raise NotImplementedError(f"astype({dt})")
-            if a.weak:
-                return self._materialise(a, dt)
+            if a.weak:  # Python evaluates it too: an int or float has no .astype
+                raise AttributeError(f"{type(a.scalar).__name__!r} object has no attribute 'astype'")
             return self._cast(a, dt)
         if not isinstance(n.func, ast.Name):
             raise NotImplementedError("only plain function names can be called in device expressions")
