@@ -89,7 +89,20 @@ def load_strings():
     return cases
 
 
-AGGLIST_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "agglist_golden.npz")
+SET_EDGES_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "set_edges_golden.npz")
+
+
+def load_set_edges():
+    """tests/golden/set_edges_golden.npz (tests/golden/make_golden_set_edges.py): case name -> dict of arrays"""
+    z = np.load(SET_EDGES_PATH, allow_pickle=False)
+    cases = {}
+    for key in z.files:
+        name, field = key.split("/", 1)
+        cases.setdefault(name, {})[field] = z[key]
+    return cases
+
+
+AGGLIST_PATH =os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "agglist_golden.npz")
 
 
 def load_agglist():

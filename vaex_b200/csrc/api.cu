@@ -953,7 +953,7 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
                     set_error("b200_bin: binner %d: hash binner without a set", i);
                     return B200_ERR_INVALID;
                 }
-                d.byteswap = 0;
+                // a non-native key column is probed by value: its bytes are swapped before the lookup (d.byteswap as set above)
                 B200_CHECK(set_fill_binner(const_cast<b200_set *>(b.set), d));
             } else {
                 d.byteswap = b.byteswap != 0; // the ordinal FlipEndian quirk flips the int64 difference, any itemsize

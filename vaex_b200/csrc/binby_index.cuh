@@ -49,15 +49,16 @@ __device__ __forceinline__ void binby_indices(const DevBinner *__restrict__ binn
         } else { // B200_BINNER_HASH: HashMapUnique.map (vaex/hash.py:193-214) + BinnerOrdinal
 #pragma unroll
             for (int j = 0; j < 4; j++) {
+                const uint64_t raw = b.byteswap ? bswap(r[j], b.isz) : r[j];
                 long long value;
                 if (j >= nv)
                     value = -1;
                 else if (m[j] == 1)
                     value = b.null_ordinal;
-                else if (raw_isnan(b.dtype, r[j]))
+                else if (raw_isnan(b.dtype, raw))
                     value = b.nan_ordinal;
                 else
-                    value = set_probe(b.table, b.table_mask, b.sentinel_ordinal, key_canon(b.dtype, r[j]));
+                    value = set_probe(b.table, b.table_mask, b.sentinel_ordinal, key_canon(b.dtype, raw));
                 idx[j] += ordinal_index(value, false, b.ordinal_count, b.allow_other != 0, b.invert != 0) * b.stride;
             }
         }

@@ -1354,6 +1354,10 @@ int str_check_error(b200_set *s, cudaStream_t st) {
     if (h[CTR_STR_ERROR]) {
         set_error(h[CTR_STR_ERROR] == 2 ? "ordered_set_string: two different strings share one 64-bit hash (std::hash collision); refusing to merge them"
                                         : "ordered_set_string: a string hashes to the reserved empty pattern");
+        // the refusal belongs to this call only: later calls that do not repeat the offending string must still succeed
+        unsigned long long zero = 0;
+        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_STR_ERROR, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
+        B200_CUDA(cudaStreamSynchronize(st));
         return B200_ERR_UNSUPPORTED;
     }
     return B200_OK;
@@ -1448,8 +1452,10 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
                                                                        in.base, nrows);
         B200_CUDA(cudaGetLastError());
     }
-    B200_CHECK(str_check_error(s, st));
+    // dirty before the error check: a refused call still inserted its other new strings (all but the offending one), and the
+    // next finalisation must see them
     s->dirty = true;
+    B200_CHECK(str_check_error(s, st));
     if (return_values && nrows) {
         B200_CHECK(str_finalize(s));
         long long *d_vals = nullptr;

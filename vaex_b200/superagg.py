@@ -153,6 +153,7 @@ class _BinnerHash(Binner):
             raise RuntimeError("data not set")
         b.kind = _lib.BINNER_HASH
         b.dtype = self._code
+        b.byteswap = int(self._non_native)
         b.ordinal_count, b.min_value = self.ordinal_count, 0
         b.allow_other, b.invert = int(self.allow_other), int(self.invert)
         b.set = self.hash_map._h
@@ -491,8 +492,7 @@ for _name in _DT:
         _common = dict(_dtype=_name, _code=_lib.DTYPE_CODE[_name], _non_native=_nn, _itemsize=_isz)
         _make("BinnerScalar_" + _sfx, _BinnerScalar, **_common)
         _make("BinnerOrdinal_" + _sfx, _BinnerOrdinal, **_common)
-        if not _nn:
-            _make("BinnerHash_" + _sfx, _BinnerHash, **_common)
+        _make("BinnerHash_" + _sfx, _BinnerHash, **_common)
         for _prefix, _op in _AGG_OPS.items():
             _make(_prefix + "_" + _sfx, Aggregator, _op=_op, **_common)
         _make("AggNUnique_" + _sfx, _AggNUnique, **_common)

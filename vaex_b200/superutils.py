@@ -53,6 +53,27 @@ class _OrderedSet:
     def _np_dtype(cls):
         return np.dtype(cls._dtype)
 
+    def _key_column(self, values):
+        """Key values as a column of the set's own dtype.  The reference takes keys as ``py::array_t<T>``
+        (src/hash_primitives.hpp:72,81,539,611), whose default forcecast converts a host array of another dtype or byte order by
+        VALUE (``update(np.array([1.7, 2.2]))`` on an int64 set inserts 1 and 2; a big-endian column inserts its numbers, not its
+        swapped bytes); host arrays get the same conversion here.  Device columns are read in place, so they must already hold
+        the set's dtype: only same-width integer types (whose bits are their values) are accepted in its stead."""
+        native = self._np_dtype()
+        cai = getattr(values, "__cuda_array_interface__", None)
+        if cai is not None and not isinstance(values, np.ndarray):
+            col = _lib.column(values)
+            dt = col.dtype
+            same_bits = dt.isnative and dt.itemsize == native.itemsize and dt.kind in "biumM" and native.kind in "biu"
+            if dt != native and not same_bits:
+                raise TypeError(f"{type(self).__name__}: a device column of dtype {dt} cannot be read as {native} keys; convert it first")
+            return col
+        a = np.asarray(values)
+        if a.dtype != native:
+            with np.errstate(invalid="ignore", over="ignore"):
+                a = a.astype(native)
+        return _lib.column(a)
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h:
@@ -76,9 +97,7 @@ class _OrderedSet:
         opts.update(kwargs)
         if opts["bucket_size"] < opts["chunk_size"]:
             raise RuntimeError("bucket size should be larger than chunk_size")
-        col = _lib.column(values)
-        if col.dtype.itemsize != self._np_dtype().itemsize:
-            raise RuntimeError("stride not equal to bytesize")
+        col = self._key_column(values)
         mcol = None
         if masks is not None:
             mcol = _lib.mask_column(masks)
@@ -146,9 +165,7 @@ class _OrderedSet:
         return out
 
     def map_ordinal(self, values):
-        col = _lib.column(values)
-        if col.dtype.itemsize != self._np_dtype().itemsize:
-            raise RuntimeError("stride not equal to bytesize for key values")
+        col = self._key_column(values)
         odt = np.dtype(_lib.DTYPES[_lib.lib().b200_set_ordinal_dtype(self._h)])
         if col.memspace == _lib.MEM_DEVICE:
             import torch
@@ -172,7 +189,7 @@ class _OrderedSet:
         return output
 
     def isin(self, values):
-        col = _lib.column(values)
+        col = self._key_column(values)
         out = np.empty(col.length, np.uint8)
         if col.memspace == _lib.MEM_DEVICE:
             import torch
