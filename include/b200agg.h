@@ -33,6 +33,8 @@
  *   b200_stat_*           TaskPartStatistic + vaexfast statisticNd_f4/_f8, every op (vaex/cpu.py:487-626, src/vaexfast.cpp:1061-1278).
  *   b200_grid_percentile  the finish of percentile_approx (vaex/dataframe.py:1675-1754) with vaexfast.grid_find_edges
  *                         (src/vaexfast.cpp:1680-1719), on a device count grid.
+ *   b200_grid_mutual_information  the finish of mutual_information (vaex/dataframe.py:766-790) with kld.mutual_information
+ *                         (vaex/kld.py:13-21), on a device count grid.
  *   b200_hash64           superutils.hash (src/superutils.cpp:265) — test hook, host only.
  */
 #ifndef B200AGG_H
@@ -288,6 +290,19 @@ int b200_stat_destroy(b200_stat *stat);
  * ndim <= B200_MAX_BINNERS. */
 int b200_grid_percentile(b200_ctx *ctx, int slot, const int64_t *grid, int ndim, const int64_t *sizes, double lb, double span, const double *pct,
                          const uint8_t *integral, int npct, int memspace_out, double *out);
+
+/* ---- mutual_information: the per-cell finish of a count grid (vaex/dataframe.py:766-790, vaex/kld.py:13-21) -----------------
+ * `grid` is a DEVICE int64 count grid with edges, first dimension fastest: the `dimension` MI axes first, the binby axes after
+ * them, `sizes` = its ndim sizes including the +3 of edges (b200_agg_device_ptr of a count(*) aggregator, a grid after an
+ * all-reduce, or any grid built by the caller).  Every axis is sliced [2:-1], as count(..., edges=False) returns it.  out[cell]
+ * receives kld.mutual_information of that binby cell's MI sub-grid, cells first binner fastest: N = the sum of the counts, the
+ * int64 marginals M_k of every MI axis, and the sum over the counts c > 0 of P * log(P / Q) with P = c / N and Q = the product of
+ * M_k / N.  An empty cell gives 0.0, dimension 1 gives exactly 0.0.  The result is run-to-run bit-identical (fixed reduction
+ * trees); against the reference's float64 numpy it holds the bound of DESIGN.md section 3, not bit equality.
+ * `out` is host memory (memspace_out = B200_MEM_HOST) or device memory (B200_MEM_DEVICE); the call waits for the result.
+ * 1 <= dimension <= ndim <= B200_MAX_BINNERS (the reference allows 16 axes, src/agg.hpp:29). */
+int b200_grid_mutual_information(b200_ctx *ctx, int slot, const int64_t *grid, int ndim, const int64_t *sizes, int dimension, int memspace_out,
+                                 double *out);
 
 /* ---- device-side expressions and filter compaction (SURVEY.md section 8f row 2) ------------------------------------------------
  * Replaces the per-chunk Python `eval` of virtual columns / filters / selections (vaex/scopes.py:108-128 _BlockScope.evaluate) and

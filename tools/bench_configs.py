@@ -2,7 +2,7 @@
 """Times every BASELINE.json configuration on one H100 with device-resident columns (the roofline setting) and prints one
 JSON object per config: rows/s, achieved algorithmic GB/s (SURVEY.md 8d bytes/row) and the fraction of the measured HBM peak.
 
-    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV,PA]
+    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV,PA,MI]
 
 This is a companion to bench.py (which owns the headline line the driver parses); results are quoted in DESIGN.md.
 """
@@ -235,6 +235,8 @@ def main():
             ls_string_list(args, ctx, stream, gen, report)
         elif cfg == "PA":
             pa_percentile(args, n, ctx, stream, gen, timed, report)
+        elif cfg == "MI":
+            mi_mutual_information(args, n, ctx, stream, gen, timed, report)
 
 
 def pa_percentile(args, n, ctx, stream, gen, timed, report):
@@ -287,6 +289,92 @@ def pa_percentile(args, n, ctx, stream, gen, timed, report):
         del a, g, out, grid
         torch.cuda.empty_cache()
     del cols
+
+
+def mi_mutual_information(args, n, ctx, stream, gen, timed, report):
+    """MI: df.mutual_information over `n` device-resident fp32 rows, y correlated with x, mi_shape=256 in [-5, 5]^2.
+    MI-pair: (x, y), one cell (a 259^2 int64 grid: the split regime).  MI-binby: the same with binby=[z], shape=128 in [-3, 3]
+    (259^2 x 131 int64 = 70 MB, 128 cells: the split regime), the device finish against the host finish the reference runs (D2H of the
+    grid into pageable memory + the numpy restatement of tests/mutual_information_oracle.py, a lower bound of the reference's per-cell
+    Python loop).  Count pass and finish are timed separately with CUDA events; each finish is checked against the restatement on
+    the same grid, within the per-cell bound of DESIGN.md section 3, before the timed runs.  MI-matrix: x=[8 columns] end to end
+    through Frame (one minmax pass per column, 36 unique pairs in one executor pass), wall clock; before the timed runs every
+    unique entry is checked against the restatement's finish of that pair's count grid."""
+    import subprocess
+    import numpy as np
+    import torch
+    from vaex_b200 import execution, frame, superagg
+    from vaex_b200 import mutual_information as _mi
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import mutual_information_oracle as MO
+    power = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    x = torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen)
+    y = x + torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen)
+    z = torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen)
+    parity = True
+    for name, nb in (("MI-pair", 0), ("MI-binby", 1)):
+        bs = [superagg.BinnerScalar_float32(1, e, -5.0, 5.0, 256) for e in "xy"] + [superagg.BinnerScalar_float32(1, "z", -3.0, 3.0, 128)][:nb]
+        g = superagg.Grid(bs)
+        for b, c in zip(bs, (x, y, z)):
+            b.set_data(0, c)
+        a = superagg.AggCount_int64(g, 1, 1)
+
+        def count():
+            a.reset(0)
+            g.bin(0, [a], n)
+        ms_count = timed(count, args.reps)
+        ptr, nbytes = a.device_pointer(0)
+        cells = 128 if nb else 1
+        out = torch.empty(cells, dtype=torch.float64, device="cuda")
+        _mi.grid_mutual_information(ptr, g.shapes, 2, ctx=ctx, out=out)
+        grid = a.get_result()[(slice(2, -1),) * (2 + nb)]
+        want, tol = (np.array([MO.mi_cell(grid[..., i].astype(np.float64)) for i in range(cells)]), np.array([MO.bound(grid[..., i]) for i in range(cells)])) \
+            if nb else (np.array([MO.mi_cell(grid.astype(np.float64))]), np.array([MO.bound(grid)]))
+        ok = int(a.get_result().sum()) == n and bool(np.all(np.abs(out.cpu().numpy() - want) <= tol))
+        parity &= ok
+        ms_finish = timed(lambda: _mi.grid_mutual_information(ptr, g.shapes, 2, ctx=ctx, out=out), args.reps)
+        host_best = d2h_best = None
+        for _ in range(max(2, args.reps // 2)):
+            t0 = time.perf_counter()
+            full = a.get_result()  # D2H into pageable memory
+            t1 = time.perf_counter()
+            MO.calculate(full[(slice(2, -1),) * (2 + nb)], nb)
+            t2 = time.perf_counter()
+            d2h_best = min(d2h_best or 1e30, (t1 - t0) * 1e3)
+            host_best = min(host_best or 1e30, (t2 - t0) * 1e3)
+        workload = "mutual_information(x, y, mi_shape=256" + (", binby=[z], shape=128" if nb else "") + ") on fp32 rows"
+        report(name + "/count", workload + ": count pass", n, 4 * (2 + nb), ms_count, gpu=power)
+        print(json.dumps(dict(config=name + "/finish", workload=workload + ": finish on the device", ms=ms_finish, grid_bytes=nbytes,
+                              grid_reads_gbs=2 * nbytes / (ms_finish * 1e-3) / 1e9, parity=ok, gpu=power)), flush=True)
+        print(json.dumps(dict(config=name + "/host_finish", workload=workload + ": D2H (pageable) + numpy finish on the host", ms=host_best,
+                              d2h_ms=d2h_best, grid_bytes=nbytes, gpu=power)), flush=True)
+        del a, g, out, grid, full
+        torch.cuda.empty_cache()
+    cols = {"x": x, "y": y, "z": z}
+    for k in range(5):
+        cols[f"c{k}"] = (x if k % 2 else z) * 0.5 + torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen)
+    f = frame.Frame(cols, executor=execution.Executor(1))
+    names = list(cols)
+    # checked before the timed runs: every unique entry against the restatement's finish of that pair's count grid (same limits)
+    m = f.mutual_information(names, mi_shape=256)
+    limits = {e: list(f.minmax(e)) for e in names}
+    ok = m.shape == (8, 8) and np.array_equal(m, m.T)
+    for i in range(8):
+        for j in range(i, 8):
+            counts = f.count(binby=[names[i], names[j]], limits=[limits[names[i]], limits[names[j]]], shape=256)
+            ok = ok and bool(abs(m[i, j] - MO.mi_cell(counts.astype(np.float64))) <= MO.bound(counts))
+    parity &= ok
+    best = None
+    for _ in range(2):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        f.mutual_information(names, mi_shape=256)
+        torch.cuda.synchronize()
+        best = min(best or 1e30, (time.perf_counter() - t0) * 1e3)
+    print(json.dumps(dict(config="MI-matrix", workload="mutual_information(x=[8 fp32 columns], mi_shape=256) end to end: 8 minmax passes (one per "
+                          "column), 36 count grids in one pass, 36 device finishes", rows=n, ms=best, parity=ok, gpu=power)), flush=True)
+    print(json.dumps(dict(config="MI", parity=bool(parity), gpu=power)), flush=True)
+    del f, cols, x, y, z
 
 
 def ls_string_list(args, ctx, stream, gen, report):

@@ -16,8 +16,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # VAEX_B200_LIB: load this build of the library instead of the in-tree one (A/B timing of kernel variants on one box)
 LIB_PATH = os.environ.get("VAEX_B200_LIB") or os.path.join(_HERE, "libb200agg.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "binby.cu", "expr.cu", "fast.cu", "first.cu", "hashset.cu", "list.cu", "minmax.cu", "nunique.cu", "percentile.cu", "ringcount.cu",
-           "statistic.cu", "tilesort.cu"]
+SOURCES = ["api.cu", "binby.cu", "expr.cu", "fast.cu", "first.cu", "hashset.cu", "list.cu", "minmax.cu", "mutinfo.cu", "nunique.cu", "percentile.cu",
+           "ringcount.cu", "statistic.cu", "tilesort.cu"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -161,6 +161,7 @@ def lib():
             "b200_stat_reset": (i32, [vp]),
             "b200_stat_destroy": (i32, [vp]),
             "b200_grid_percentile": (i32, [vp, i32, vp, i32, P(i64), C.c_double, C.c_double, P(C.c_double), P(C.c_uint8), i32, i32, vp]),
+            "b200_grid_mutual_information": (i32, [vp, i32, vp, i32, P(i64), i32, i32, vp]),
             "b200_host_register": (i32, [vp, sz]),
             "b200_host_unregister": (i32, [vp]),
             "b200_hash64": (u64, [u64]),

@@ -80,6 +80,26 @@ static __device__ __forceinline__ long long block_exclusive_i64(long long v, lon
     return before + x - v;
 }
 
+// sum of one value per thread over a kScanThreads block in a fixed tree (xor butterfly per warp, then the warp sums in warp order),
+// so a floating-point sum is the same bits on every run; every thread receives it.  Ends with a barrier: callable in a loop.
+template <typename T>
+static __device__ __forceinline__ T block_sum(T v) {
+    __shared__ T warp_sums[kScanThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0)
+        warp_sums[warp] = v;
+    __syncthreads();
+    T all = warp_sums[0];
+#pragma unroll
+    for (int w = 1; w < kScanThreads / 32; w++)
+        all += warp_sums[w];
+    __syncthreads();
+    return all;
+}
+
 static __global__ void __launch_bounds__(kScanThreads) k_scan_i64_sums(const long long *a, unsigned long long n, long long *sums) {
     const unsigned long long i0 = blockIdx.x * kScanTile + (unsigned long long)threadIdx.x * kScanItems;
     long long s = 0;

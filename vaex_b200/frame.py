@@ -279,11 +279,20 @@ class Frame:
             return self._limit(expressions, value, selection)
         return np.array(self._limits_list(expressions, value, selection))
 
-    def _limits_list(self, expressions, value, selection):
-        if value is None:
-            value = "minmax"
-        values = (value,) * len(expressions) if _is_limit(value) or not _issequence(value) else value
-        return [self._limit(e, v, selection) for e, v in zip(expressions, values)]
+    def _limits_list(self, expressions, value, selection, memo=None):
+        """one limit per expression; with `memo` (a dict kept over one call), an expression's "minmax" / "N%" limit is computed
+        once however many lists name it, as vaex keys its limit tasks by (expression, value) (vaex/dataframe.py:1903-1905)"""
+        values = _per_expression("minmax" if value is None else value, len(expressions))
+        out = []
+        for e, v in zip(expressions, values):
+            if memo is None or _is_limit(v) or not isinstance(v, (str, type(None))):
+                out.append(self._limit(e, v, selection))
+                continue
+            key = (e, "minmax" if v is None else v, selection)
+            if key not in memo:
+                memo[key] = self._limit(e, v, selection)
+            out.append(memo[key])
+        return out
 
     def _limit(self, expression, value, selection=None):
         if _is_limit(value):
@@ -300,7 +309,7 @@ class Frame:
         """df.limits_percentage (vaex/dataframe.py:1795-1842): a range around the median holding about `percentage` % of the rows, read
         off the normalised cumulative counts of a 16384-bin count between the minmax limits (np.interp on the host)"""
         from . import percentile as _pct
-        waslist, expressions = _pct.listify(expression)
+        waslist, (expressions,) = _pct.listify(expression)
         out = []
         for e in expressions:
             limits_minmax = self.minmax(e, selection=selection)
@@ -323,7 +332,7 @@ class Frame:
         and finished on the device.  With two or more binby dimensions each cell gets the answer of the reference's one-dimensional
         code for that cell (DESIGN.md section 3)."""
         from . import percentile as _pct
-        waslist, expressions = _pct.listify(expression)
+        waslist, (expressions,) = _pct.listify(expression)
         expressions = [str(e) for e in expressions]
         binby = [] if binby is None else ([binby] if not isinstance(binby, (list, tuple)) else list(binby))
         selection = None if selection is False else selection
@@ -368,6 +377,74 @@ class Frame:
         there), 256 percentile bins by default"""
         return self.percentile_approx(expression, 50, binby=binby, limits=limits, shape=shape, percentile_shape=percentile_shape,
                                       percentile_limits=percentile_limits, selection=selection)
+
+    # ---- mutual information: count passes, the per-cell finish on the device (csrc/mutinfo.cu) --------------------------------
+    def mutual_information(self, x, y=None, dimension=2, mi_limits=None, mi_shape=256, binby=[], limits=None, shape=128, sort=False,
+                           selection=False):
+        """df.mutual_information (vaex/dataframe.py:685-819) between x and y, a list of pairs, a `dimension`-axis matrix over x or the
+        x by y matrix, on an `mi_shape` grid between `mi_limits`, optionally per cell of a binby grid (at most 3 axes).  Every unique
+        combination is one count(*) grid finished on the device; the combinations of a call share executor passes, as many per pass
+        as fit the grid budget of mutual_information.py.  The reference's result shapes and quirks are kept (DESIGN.md section 3);
+        a string `binby` is one expression."""
+        from . import mutual_information as _mi
+        combinations, shape_result, waslist, mi_limits = _mi.plan(x, y, dimension, mi_limits)
+        binby = [binby] if isinstance(binby, str) else list(binby)
+        if len(binby) > 3:
+            raise ValueError("binby with dim > 3 is not yet supported")
+        binby = [str(b) for b in binby]
+        selection = None if selection is False else selection
+        binby_shape = _expand_shape(shape, len(binby))
+        combinations_unique, unique_reverse = _mi.unique_combinations(combinations)
+        f = self
+        names = list(dict.fromkeys([str(e) for c in combinations_unique for e in c] + binby))
+        missing = [e for e in names if e not in self.columns]
+        if missing:
+            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
+            for e in missing:
+                f.columns[e] = f.expression(e)
+        for e in names:
+            if e in f.categories or _dtype_of(f.columns[e]).kind in "mMO":
+                raise NotImplementedError(f"mutual_information over the categorical, datetime or string column {e!r} is not supported")
+        # the limits come from all rows of the frame, not the selection's (:762, :769), and every name's minmax once per call
+        memo = {}
+        binby_limits = f._limits_list(binby, limits, None, memo)
+        values = _per_expression(mi_limits, len(combinations_unique))
+        combination_limits = [f._limits_list([str(e) for e in c], v, None, memo) for c, v in zip(combinations_unique, values)]
+        mask = f.expression(selection) if isinstance(selection, str) else selection
+        if isinstance(selection, str) and mask.dtype != np.bool_:
+            raise ValueError("a selection must be a boolean expression")
+        dtypes = f.dtypes()
+        nthreads = f.executor.nthreads
+
+        def spec(e, count, lim):
+            return {"binner-type": "scalar", "expression": e, "dtype": dtypes[e].str, "count": int(count), "minimum": float(lim[0]),
+                    "maximum": float(lim[1])}
+        plans = []
+        for c, lims in zip(combinations_unique, combination_limits):
+            c = [str(e) for e in c]
+            specs = [spec(e, n, lim) for e, n, lim in zip(c, _expand_shape(mi_shape, len(c)), lims)]
+            specs += [spec(b, n, lim) for b, n, lim in zip(binby, binby_shape, binby_limits)]
+            plans.append((len(c), specs, 8 * int(np.prod([s["count"] + 3 for s in specs], dtype=np.int64))))
+        budget, free = _mi.grid_budget(_lib.context().device)
+        for (_, specs, nbytes), c in zip(plans, combinations_unique):
+            if nbytes > free:
+                shape_ = tuple(s["count"] for s in specs)
+                raise MemoryError(f"mutual_information of {c}: the count grid of shape {shape_} (with edges, {nbytes} bytes) exceeds the "
+                                  f"{free} bytes free on the device")
+        mi_list = []
+        for batch in _mi.batches([p[2] for p in plans], budget):
+            tasks = []
+            for i in batch:
+                d, specs, _ = plans[i]
+                desc = _agg.count("*", selection=None if mask is None else "selection", edges=True)
+                desc._prepare_types(dtypes)
+                part = taskpart.TaskPartMutualInformation(None, [taskpart.decode_binner(s, nthreads) for s in specs], [desc], dtypes, d,
+                                                          nthreads=nthreads)
+                tasks.append(execution.Task(part, [mask]))
+            f.executor.execute(f.columns, tasks, f.length, filter=f._filter)
+            mi_list += [t.result for t in tasks]
+            del tasks, part  # the batch's count grids go back before the next batch allocates
+        return _mi.assemble(mi_list, x, unique_reverse, binby_shape, shape_result, waslist, sort)
 
     # ---- binned statistics -------------------------------------------------------------------------------------------
     def _binner_specs(self, binby, limits, shape):
@@ -707,6 +784,11 @@ class GroupBy:
 
 def _issequence(x):
     return isinstance(x, (tuple, list, np.ndarray))
+
+
+def _per_expression(value, n):
+    """df.limits' broadcast: one limit value (a pair, a string or None) for all n expressions, else one per expression"""
+    return (value,) * n if _is_limit(value) or not _issequence(value) else value
 
 
 def _is_limit(x):

@@ -8,20 +8,25 @@ import numpy as np
 from . import _lib
 
 
-def listify(x):
-    """vaex.utils.listify for one argument: (waslist, items)"""
-    if isinstance(x, str):
-        return False, [x]
+def listify(*args):
+    """vaex.utils.listify: (True, args) when the first argument is a sequence, else (False, [[a] for a in args]); unpack one
+    argument as ``waslist, (items,) = listify(x)``"""
+    if isinstance(args[0], str):
+        return False, [[x] for x in args]
     try:
-        x[0]
-        return True, x
+        args[0][0]
+        return True, args
     except Exception:
-        return False, [x]
+        return False, [[x] for x in args]
 
 
-def unlistify(waslist, x):
-    """vaex.utils.unlistify for one argument"""
-    return x if waslist else x[0]
+def unlistify(waslist, *args):
+    """vaex.utils.unlistify: the inverse of listify (None for several arguments that were not lists, as there)"""
+    if waslist:
+        return args[0] if len(args) == 1 else args
+    values = [x[0] for x in args]
+    if len(values) == 1:
+        return values[0]
 
 
 def is_integral(p):
@@ -53,7 +58,7 @@ def finish(grid_ptr, sizes, limit, percentage, ctx=None, slot=0):
     """One expression's result of the reference's finish (vaex/dataframe.py:1677-1752) from the count grid at `grid_ptr`: per
     percentage a scalar limit (0 or 100) or the grid of sliced binby cells (a numpy scalar without binby), stacked with np.array and
     unlistified over the percentages."""
-    waslist, percentages = listify(percentage)
+    waslist, (percentages,) = listify(percentage)
     lb, ub = limit
     with np.errstate(all="ignore"):
         span = ub - lb  # in the limits' dtype: a float32 minmax gives a float32 span

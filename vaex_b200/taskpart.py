@@ -226,6 +226,28 @@ class TaskPartPercentile(TaskPartAggregation):
         return _pct.finish(ptr, self.grid.shapes, self.limit, self.percentage, op._ctx)
 
 
+class TaskPartMutualInformation(TaskPartAggregation):
+    """mutual_information of one combination (vaex/dataframe.py:685-819): the count(*) pass over combination + binby with edges
+    (:796-797) on one device grid, then the per-cell finish on that grid (csrc/mutinfo.cu).  Only one double per binby cell is read
+    back; the count grid never leaves the device.  ``dimension`` is the number of leading MI axes."""
+    snake_name = "mutual_information"
+
+    def __init__(self, df, binners, aggregation_descriptions, dtypes, dimension, nthreads=None):
+        super().__init__(df, binners, aggregation_descriptions, dtypes, nthreads=nthreads)
+        (desc, selections, ops, _), = self.aggregations
+        if len(ops) != 1 or desc.expressions:
+            raise ValueError("a mutual information task part holds one count(*) aggregator with one selection")
+        self.dimension = int(dimension)
+
+    def get_result(self):
+        from . import mutual_information as _mi
+        op = self.aggregations[0][2][0]
+        if op.device_dtype != np.int64:
+            raise RuntimeError("the mutual information finish reads an int64 count grid")
+        ptr, _ = op.device_pointer(0)
+        return _mi.finish(ptr, self.grid.shapes, self.dimension, op._ctx)
+
+
 class RowLimitException(ValueError):
     pass
 
