@@ -150,6 +150,9 @@ int b200_ctx_path_stats(b200_ctx *ctx, int slot, uint64_t out[6]);
  * waiting for a free piece of the page-locked bounce ring, in memcpy into the ring, enqueueing the pieces' copies, and in b200_bin
  * as a whole; out[4] pieces copied, out[5] calls.  reset != 0 zeroes the counters.  No reference counterpart (instrumentation). */
 int b200_ctx_host_stats(b200_ctx *ctx, uint64_t out[6], int reset);
+/* Device memory of the context's block cache, in bytes: out[0] handed out and not yet returned (grids, sets, statistics and per-call
+ * temporaries; the slots' staging and partition arenas are not counted), out[1] held idle in the cache.  No reference counterpart. */
+int b200_ctx_mem_stats(b200_ctx *ctx, uint64_t out[2]);
 /* Measurement aid: enqueue on `slot`'s stream a kernel of `ctas` CTAs x `threads` threads with `smem_bytes` of shared memory that
  * does nothing for `nanoseconds` — it stands in for another stream's kernel holding SMs (an NCCL all-reduce) so that one GPU can
  * show what that costs a persistent kernel on a different slot (tools/ab_headline.py --occupy).  No reference counterpart. */

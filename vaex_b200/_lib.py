@@ -106,6 +106,7 @@ def lib():
             "b200_ctx_stream": (i32, [vp, i32, P(vp)]),
             "b200_ctx_path_stats": (i32, [vp, i32, P(u64)]),
             "b200_ctx_host_stats": (i32, [vp, P(u64), i32]),
+            "b200_ctx_mem_stats": (i32, [vp, P(u64)]),
             "b200_ctx_occupy": (i32, [vp, i32, i32, i32, i32, u64]),
             "b200_agg_create": (i32, [vp, i32, i32, i32, i32, u32, u64, P(vp)]),
             "b200_agg_destroy": (i32, [vp]),
@@ -218,6 +219,12 @@ class Context:
         out = (C.c_uint64 * 6)()
         check(lib().b200_ctx_host_stats(self._h, out, int(bool(reset))))
         return dict(wait_ms=out[0] / 1e6, memcpy_ms=out[1] / 1e6, enqueue_ms=out[2] / 1e6, bin_ms=out[3] / 1e6, pieces=out[4], calls=out[5])
+
+    def mem_stats(self):
+        """Bytes of the context's block cache (include/b200agg.h b200_ctx_mem_stats): handed out and not returned, and held idle."""
+        out = (C.c_uint64 * 2)()
+        check(lib().b200_ctx_mem_stats(self._h, out))
+        return dict(live=out[0], cached=out[1])
 
     def stream(self, slot=0):
         s = C.c_void_p()

@@ -87,19 +87,21 @@ static size_t cache_class(size_t bytes) {
     return align_up(bytes, step);
 }
 
-cudaError_t ctx_alloc(b200_ctx *ctx, void **out, size_t bytes) {
-    bytes = cache_class(bytes);
+int ctx_alloc(b200_ctx *ctx, void **out, size_t bytes, const char *what) {
+    const size_t cls = cache_class(bytes);
     {
         std::lock_guard<std::mutex> g(ctx->cache_mu);
-        auto it = ctx->cache.find(bytes);
+        auto it = ctx->cache.find(cls);
         if (it != ctx->cache.end()) {
             *out = it->second;
             ctx->cache.erase(it);
-            ctx->cache_bytes -= bytes;
-            return cudaSuccess;
+            ctx->cache_bytes -= cls;
+            ctx->live_bytes += cls;
+            return B200_OK;
         }
     }
-    cudaError_t e = cudaMalloc(out, bytes);
+    *out = nullptr;
+    cudaError_t e = cudaMalloc(out, cls);
     if (e == cudaErrorMemoryAllocation) { // give the cache back before reporting out-of-memory
         cudaGetLastError();
         std::lock_guard<std::mutex> g(ctx->cache_mu);
@@ -107,18 +109,29 @@ cudaError_t ctx_alloc(b200_ctx *ctx, void **out, size_t bytes) {
             cudaFree(kv.second);
         ctx->cache.clear();
         ctx->cache_bytes = 0;
-        e = cudaMalloc(out, bytes);
+        e = cudaMalloc(out, cls);
     }
-    return e;
+    if (e == cudaErrorMemoryAllocation) {
+        cudaGetLastError();
+        *out = nullptr;
+        set_error("%s: out of device memory for %zu bytes", what, bytes);
+        return B200_ERR_NOMEM;
+    }
+    if (e != cudaSuccess) {
+        *out = nullptr;
+        return cuda_fail(e, what, __FILE__, __LINE__);
+    }
+    std::lock_guard<std::mutex> g(ctx->cache_mu);
+    ctx->live_bytes += cls;
+    return B200_OK;
 }
 
 void ctx_release(b200_ctx *ctx, void *p, size_t bytes) {
-    if (!p)
-        return;
     bytes = cache_class(bytes);
     constexpr size_t kCacheLimit = 4ull << 30; // per context; a block larger than a quarter of it is never kept
     {
         std::lock_guard<std::mutex> g(ctx->cache_mu);
+        ctx->live_bytes -= bytes;
         if (bytes <= kCacheLimit / 4 && ctx->cache_bytes + bytes <= kCacheLimit) {
             ctx->cache.emplace(bytes, p);
             ctx->cache_bytes += bytes;
@@ -518,10 +531,18 @@ int b200_ctx_host_stats(b200_ctx *ctx, uint64_t out[6], int reset) {
     return B200_OK;
 }
 
+int b200_ctx_mem_stats(b200_ctx *ctx, uint64_t out[2]) {
+    if (!ctx || !out) {
+        set_error("b200_ctx_mem_stats: invalid argument");
+        return B200_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> g(ctx->cache_mu);
+    out[0] = ctx->live_bytes, out[1] = ctx->cache_bytes;
+    return B200_OK;
+}
+
 // ---- aggregators -----------------------------------------------------------------------------------
 static bool is_list(int op) { return op == B200_AGG_LIST || op == B200_AGG_LIST_STRING; }
-static size_t agg_cells_alloc(const b200_agg *a) { return is_list(a->op) ? 16 : (a->cells ? a->cells : 1); }
-static size_t agg_grid_bytes(const b200_agg *a) { return agg_cells_alloc(a) * dtype_size(a->cell_dtype) * (a->op == B200_AGG_NUNIQUE ? 3 : 1); }
 
 int b200_agg_create(b200_ctx *ctx, int op, int dtype, int dtype2, int byteswap, uint32_t moment, uint64_t cells, b200_agg **out) {
     if (!ctx || !out || op < B200_AGG_COUNT || op > B200_AGG_LIST_STRING || dtype < 0 || dtype >= B200_NDTYPE || dtype2 < 0 || dtype2 >= B200_NDTYPE) {
@@ -529,7 +550,7 @@ int b200_agg_create(b200_ctx *ctx, int op, int dtype, int dtype2, int byteswap, 
         return B200_ERR_INVALID;
     }
     B200_CUDA(cudaSetDevice(ctx->device));
-    b200_agg *a = new b200_agg;
+    std::unique_ptr<b200_agg, int (*)(b200_agg *)> a(new b200_agg, b200_agg_destroy);
     a->ctx = ctx;
     a->op = op;
     a->dtype = dtype;
@@ -549,36 +570,20 @@ int b200_agg_create(b200_ctx *ctx, int op, int dtype, int dtype2, int byteswap, 
     default: a->cell_dtype = dtype; break;
     }
     const size_t n = is_list(op) ? 16 : (cells ? cells : 1);
-    cudaError_t e = ctx_alloc(ctx, &a->grid, agg_grid_bytes(a));
-    if (e == cudaSuccess && op == B200_AGG_NUNIQUE)
-        e = cudaMalloc((void **)&a->ntotal, 8);
-    if (e == cudaSuccess && (op == B200_AGG_FIRST || op == B200_AGG_LAST)) {
-        e = ctx_alloc(ctx, &a->state, n * 16);
-        if (e == cudaSuccess)
-            e = ctx_alloc(ctx, &a->order, n * dtype_size(dtype2));
-        if (e == cudaSuccess)
-            e = ctx_alloc(ctx, (void **)&a->cell_masked, n);
-        if (e == cudaSuccess)
-            e = cudaEventCreateWithFlags(&a->chain, cudaEventDisableTiming);
-    }
-    if (e != cudaSuccess) {
-        b200_agg_destroy(a);
-        if (e == cudaErrorMemoryAllocation) {
-            cudaGetLastError();
-            set_error("b200_agg_create: out of device memory for %llu cells", (unsigned long long)cells);
-            return B200_ERR_NOMEM;
-        }
-        return cuda_fail(e, "cudaMalloc(grid)", __FILE__, __LINE__);
+    const size_t grid_bytes = n * dtype_size(a->cell_dtype) * (op == B200_AGG_NUNIQUE ? 3 : 1);
+    B200_CHECK(a->grid.alloc(ctx, grid_bytes, "b200_agg_create"));
+    if (op == B200_AGG_NUNIQUE)
+        B200_CHECK(a->ntotal.alloc(ctx, 8, "b200_agg_create"));
+    if (op == B200_AGG_FIRST || op == B200_AGG_LAST) {
+        B200_CHECK(a->state.alloc(ctx, n * 16, "b200_agg_create"));
+        B200_CHECK(a->order.alloc(ctx, n * dtype_size(dtype2), "b200_agg_create"));
+        B200_CHECK(a->cell_masked.alloc(ctx, n, "b200_agg_create"));
+        B200_CUDA(cudaEventCreateWithFlags(&a->chain, cudaEventDisableTiming));
     }
     cudaStream_t st = ctx->slots[0]->stream;
-    int rc = agg_fill(a, st);
-    if (!rc && cudaStreamSynchronize(st) != cudaSuccess)
-        rc = B200_ERR_CUDA;
-    if (rc) {
-        b200_agg_destroy(a);
-        return rc;
-    }
-    *out = a;
+    B200_CHECK(agg_fill(a.get(), st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    *out = a.release();
     return B200_OK;
 }
 
@@ -586,26 +591,9 @@ int b200_agg_destroy(b200_agg *a) {
     if (!a)
         return B200_OK;
     cudaSetDevice(a->ctx->device);
-    // the cell-shaped buffers go back to the context's cache: nothing in flight may still touch them
+    // the buffers go back to the context's cache: nothing in flight may still touch them
     for (Slot *s : a->ctx->slots)
         cudaStreamSynchronize(s->stream);
-    const size_t n = agg_cells_alloc(a);
-    ctx_release(a->ctx, a->grid, agg_grid_bytes(a));
-    ctx_release(a->ctx, a->state, n * 16);
-    ctx_release(a->ctx, a->order, n * dtype_size(a->dtype2));
-    ctx_release(a->ctx, a->cell_masked, n);
-    cudaFree(a->ntable);
-    cudaFree(a->ntotal);
-    cudaFree(a->list_keys);
-    cudaFree(a->list_vals);
-    cudaFree(a->list_counts);
-    cudaFree(a->list_starts);
-    cudaFree(a->lstr_pool);
-    cudaFree(a->lstr_off);
-    cudaFree(a->lstr_bytes);
-    cudaFree(a->lstr_valid);
-    if (a->chain)
-        cudaEventDestroy(a->chain);
     delete a;
     return B200_OK;
 }
@@ -783,13 +771,6 @@ int b200_agg_write(b200_agg *a, const void *values) {
     return B200_OK;
 }
 
-namespace {
-struct DeviceTemp {
-    void *p = nullptr;
-    ~DeviceTemp() { cudaFree(p); }
-};
-} // namespace
-
 int b200_agg_merge(b200_agg *a, b200_agg *const *others, int nothers) {
     if (!a || (nothers && !others)) {
         set_error("b200_agg_merge: invalid argument");
@@ -813,38 +794,29 @@ int b200_agg_merge(b200_agg *a, b200_agg *const *others, int nothers) {
         if (o->ctx != a->ctx)
             B200_CHECK(b200_ctx_sync(o->ctx, -1));
         // same-process peers on other devices are read through UVA peer access when enabled; keep it simple: stage through host
-        const void *src = o->grid;
-        DeviceTemp tmp_, tstate_, torder_, tmask_; // freed on every way out of this iteration
-        void *&tmp = tmp_.p, *&tstate = tstate_.p, *&torder = torder_.p, *&tmask = tmask_.p;
-        b200_agg view; // shallow alias of `o` (b200_agg is not copyable: it owns a mutex)
-        view.ctx = o->ctx, view.op = o->op, view.dtype = o->dtype, view.dtype2 = o->dtype2, view.byteswap = o->byteswap, view.moment = o->moment;
-        view.cells = o->cells, view.cell_dtype = o->cell_dtype, view.grid = o->grid, view.state = o->state, view.order = o->order, view.cell_masked = o->cell_masked;
+        FirstGrids src{o->grid, o->state, o->order, o->cell_masked};
+        DevBuf<> tgrid, tstate, torder; // peer copies, freed on every way out of this iteration
+        DevBuf<uint8_t> tmask;
         if (o->ctx->device != a->ctx->device) {
             const size_t nb = o->cells * dtype_size(o->cell_dtype);
-            B200_CUDA(cudaMalloc(&tmp, nb ? nb : 1));
-            B200_CUDA(cudaMemcpyPeer(tmp, a->ctx->device, o->grid, o->ctx->device, nb));
-            src = tmp;
-            view.grid = tmp;
+            B200_CHECK(tgrid.alloc(a->ctx, nb, "b200_agg_merge", st));
+            B200_CUDA(cudaMemcpyPeerAsync(tgrid, a->ctx->device, o->grid, o->ctx->device, nb, st));
+            src.grid = tgrid;
             if (o->state) {
-                B200_CUDA(cudaMalloc(&tstate, o->cells * 16));
-                B200_CUDA(cudaMemcpyPeer(tstate, a->ctx->device, o->state, o->ctx->device, o->cells * 16));
-                B200_CUDA(cudaMalloc(&torder, o->cells * dtype_size(o->dtype2)));
-                B200_CUDA(cudaMemcpyPeer(torder, a->ctx->device, o->order, o->ctx->device, o->cells * dtype_size(o->dtype2)));
-                B200_CUDA(cudaMalloc(&tmask, o->cells));
-                B200_CUDA(cudaMemcpyPeer(tmask, a->ctx->device, o->cell_masked, o->ctx->device, o->cells));
-                view.state = tstate;
-                view.order = torder;
-                view.cell_masked = static_cast<uint8_t *>(tmask);
+                B200_CHECK(tstate.alloc(a->ctx, o->cells * 16, "b200_agg_merge", st));
+                B200_CUDA(cudaMemcpyPeerAsync(tstate, a->ctx->device, o->state, o->ctx->device, o->cells * 16, st));
+                B200_CHECK(torder.alloc(a->ctx, o->cells * dtype_size(o->dtype2), "b200_agg_merge", st));
+                B200_CUDA(cudaMemcpyPeerAsync(torder, a->ctx->device, o->order, o->ctx->device, o->cells * dtype_size(o->dtype2), st));
+                B200_CHECK(tmask.alloc(a->ctx, o->cells, "b200_agg_merge", st));
+                B200_CUDA(cudaMemcpyPeerAsync(tmask, a->ctx->device, o->cell_masked, o->ctx->device, o->cells, st));
+                src.state = tstate, src.order = torder, src.cell_masked = tmask;
             }
         }
-        int rc;
         if (a->op == B200_AGG_FIRST || a->op == B200_AGG_LAST)
-            rc = launch_merge_first(st, a, &view);
+            B200_CHECK(launch_merge_first(st, a, src));
         else
-            rc = launch_merge(st, a->op, a->cell_dtype, a->grid, src, a->cells);
-        if (!rc && cudaStreamSynchronize(st) != cudaSuccess)
-            rc = B200_ERR_CUDA;
-        B200_CHECK(rc);
+            B200_CHECK(launch_merge(st, a->op, a->cell_dtype, a->grid, src.grid, a->cells));
+        B200_CUDA(cudaStreamSynchronize(st));
     }
     return B200_OK;
 }
@@ -866,7 +838,7 @@ static int bin_nunique(b200_ctx *ctx, Slot *sl, b200_agg *a, const DevBinner *db
     np.data = data;
     np.valid = valid;
     np.selection = selection;
-    np.distinct = static_cast<unsigned long long *>(a->grid);
+    np.distinct = static_cast<unsigned long long *>(a->grid.get());
     np.nan_rows = np.distinct + a->cells;
     np.null_rows = np.distinct + 2 * a->cells;
     np.total = a->ntotal;
@@ -878,20 +850,17 @@ static int bin_nunique(b200_ctx *ctx, Slot *sl, b200_agg *a, const DevBinner *db
         while (need < 2 * (a->npairs + (uint64_t)n))
             need <<= 1;
         if (need > a->ncap) {
-            unsigned long long *nt = nullptr;
-            cudaError_t e = cudaMalloc((void **)&nt, need * 16);
-            if (e != cudaSuccess) {
-                cudaGetLastError();
-                set_error("nunique: out of device memory for a table of %llu slots", (unsigned long long)need);
-                return B200_ERR_NOMEM;
-            }
+            // the old table goes back to the cache once the rehash has drained `st`: every other launch that reads it ran under
+            // a->nmu and was synchronised before the lock was released (below)
+            DevBuf<unsigned long long> nt;
+            B200_CHECK(nt.alloc(ctx, need * 16, "nunique", st));
             B200_CUDA(cudaMemsetAsync(nt, 0xff, need * 16, st));
             if (a->ntable) {
                 B200_CHECK(launch_nunique_rehash(st, a->ntable, a->ncap, nt, need));
                 B200_CUDA(cudaStreamSynchronize(st));
-                cudaFree(a->ntable);
             }
-            a->ntable = nt;
+            nt.unbind();
+            a->ntable = std::move(nt);
             a->ncap = need;
         }
         np.table = a->ntable;
@@ -1087,7 +1056,7 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
             fp.mask = static_cast<const uint8_t *>(stg.dev(aggs[k].mask));
             fp.grid = a->grid;
             fp.order_grid = a->order;
-            fp.state = static_cast<unsigned long long *>(a->state);
+            fp.state = static_cast<unsigned long long *>(a->state.get());
             fp.cell_masked = a->cell_masked;
             bool v = vec && !(reinterpret_cast<uintptr_t>(fp.data) & 15) && !(reinterpret_cast<uintptr_t>(fp.order) & 15);
             // select+deposit of one aggregator must not interleave with another slot's pair on the same grid: pairs are chained

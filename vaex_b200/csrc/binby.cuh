@@ -164,6 +164,11 @@ int launch_first(b200_ctx *ctx, cudaStream_t stream, const FirstParams &p, bool 
 int launch_fill(cudaStream_t stream, void *ptr, int cell_dtype, uint64_t cells, uint64_t bits);
 int launch_fill_elems(cudaStream_t stream, void *ptr, int isz, uint64_t n, uint64_t bits);
 int launch_merge(cudaStream_t stream, int op, int cell_dtype, void *dst, const void *src, uint64_t cells);
-int launch_merge_first(cudaStream_t stream, b200_agg *dst, const b200_agg *src);
+// the FIRST/LAST state merged into an aggregator: another aggregator's buffers, or copies of them on this device
+struct FirstGrids {
+    const void *grid, *state, *order;
+    const uint8_t *cell_masked;
+};
+int launch_merge_first(cudaStream_t stream, b200_agg *dst, const FirstGrids &src);
 
 } // namespace b200

@@ -6,8 +6,10 @@
 #include <string.h>
 
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200agg.h"
@@ -101,6 +103,59 @@ struct Slot {
     std::mutex mu;
 };
 
+// ---- device memory -----------------------------------------------------------------------------
+// The context's block cache (api.cu), called only by DevBuf.  ctx_alloc takes a cached block of the size class or cudaMalloc's one;
+// when the device is full it gives the cache back and retries, and reports B200_ERR_NOMEM naming `what` and the size.
+int ctx_alloc(b200_ctx *ctx, void **out, size_t bytes, const char *what);
+void ctx_release(b200_ctx *ctx, void *p, size_t bytes);
+
+// One block of device memory from the context's cache, owned by exactly one handle: the block goes back to the cache, filed under the
+// size it was allocated with, when the handle is reset, assigned to or destroyed.  A handle bound to a stream waits for that stream
+// first: per-call temporaries are bound to the stream that uses them, so an early return cannot hand a block that a kernel or copy
+// still uses to the next caller.  Unbound handles belong to objects whose *_destroy synchronises every slot before deleting them.
+template <typename T = void> class DevBuf {
+  public:
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept { *this = std::move(o); }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        if (this != &o) {
+            reset();
+            ctx_ = o.ctx_, ptr_ = o.ptr_, bytes_ = o.bytes_, stream_ = o.stream_, bound_ = o.bound_;
+            o.ptr_ = nullptr;
+        }
+        return *this;
+    }
+    ~DevBuf() { reset(); }
+
+    int alloc(b200_ctx *ctx, size_t bytes, const char *what) { return alloc(ctx, bytes, what, nullptr, false); }
+    int alloc(b200_ctx *ctx, size_t bytes, const char *what, cudaStream_t st) { return alloc(ctx, bytes, what, st, true); }
+    // the bound stream has been synchronised and the block now belongs to an object
+    void unbind() { bound_ = false; }
+    void reset() {
+        if (!ptr_)
+            return;
+        if (bound_)
+            cudaStreamSynchronize(stream_);
+        ctx_release(ctx_, ptr_, bytes_);
+        ptr_ = nullptr;
+    }
+    T *get() const { return static_cast<T *>(ptr_); }
+    operator T *() const { return get(); }
+
+  private:
+    int alloc(b200_ctx *ctx, size_t bytes, const char *what, cudaStream_t st, bool bound) {
+        reset();
+        B200_CHECK(ctx_alloc(ctx, &ptr_, bytes, what));
+        ctx_ = ctx, bytes_ = bytes, stream_ = st, bound_ = bound;
+        return B200_OK;
+    }
+    b200_ctx *ctx_ = nullptr;
+    void *ptr_ = nullptr;
+    size_t bytes_ = 0;
+    cudaStream_t stream_ = nullptr;
+    bool bound_ = false;
+};
+
 } // namespace b200
 
 struct b200_ctx {
@@ -116,6 +171,7 @@ struct b200_ctx {
     std::mutex cache_mu;
     std::multimap<size_t, void *> cache;
     size_t cache_bytes = 0;
+    size_t live_bytes = 0; // handed out and not yet returned (b200_ctx_mem_stats)
 };
 
 struct b200_agg {
@@ -123,35 +179,40 @@ struct b200_agg {
     int op = 0, dtype = 0, dtype2 = 0, byteswap = 0;
     uint32_t moment = 0;
     uint64_t cells = 0;
-    int cell_dtype = 0;     // device cell type of `grid`
-    void *grid = nullptr;   // cells * dtype_size(cell_dtype)
-    void *state = nullptr;  // FIRST/LAST: cells * 16 B {u64 order key, u64 global row}
-    void *order = nullptr;  // FIRST/LAST: cells * dtype_size(dtype2) raw order values
-    uint8_t *cell_masked = nullptr; // FIRST/LAST
-    cudaEvent_t chain = nullptr;    // FIRST/LAST: completion of the previous select+deposit pair on this grid (any slot)
+    int cell_dtype = 0;        // device cell type of `grid`
+    b200::DevBuf<> grid;       // cells * dtype_size(cell_dtype)
+    b200::DevBuf<> state;      // FIRST/LAST: cells * 16 B {u64 order key, u64 global row}
+    b200::DevBuf<> order;      // FIRST/LAST: cells * dtype_size(dtype2) raw order values
+    b200::DevBuf<uint8_t> cell_masked; // FIRST/LAST
+    cudaEvent_t chain = nullptr;       // FIRST/LAST: completion of the previous select+deposit pair on this grid (any slot)
     std::mutex chain_mu;
     // NUNIQUE: `grid` holds three planes of `cells` u64 (distinct pairs, NaN rows, null rows); the distinct (cell, value) pairs
     // live in one open-addressing table of 16-byte slots
-    unsigned long long *ntable = nullptr;
-    uint64_t ncap = 0;                     // slots (power of two)
-    unsigned long long *ntotal = nullptr;  // device counter: pairs in the table
-    uint64_t npairs = 0;                   // host copy, refreshed after every launch
-    std::mutex nmu;                        // growth needs the table to itself
+    b200::DevBuf<unsigned long long> ntable;
+    uint64_t ncap = 0;                       // slots (power of two)
+    b200::DevBuf<unsigned long long> ntotal; // device counter: pairs in the table
+    uint64_t npairs = 0;                     // host copy, refreshed after every launch
+    std::mutex nmu;                          // growth needs the table to itself
     // LIST (list.cu): one record per row {cell * 4 + category, value bits}, appended per call, sorted when the result is asked for
-    unsigned long long *list_keys = nullptr, *list_vals = nullptr;
-    unsigned *list_counts = nullptr;       // after finish: exclusive offsets per cell (+ the total)
+    b200::DevBuf<unsigned long long> list_keys, list_vals;
+    b200::DevBuf<unsigned> list_counts; // after finish: exclusive offsets per cell (+ the total)
     uint64_t list_n = 0, list_cap = 0, list_total = 0;
     bool list_sorted = false;
     // LIST_STRING (list.cu): the same records (key = cell, payload = record index | null << 63); every call appends its byte range
     // to `lstr_pool` and list_starts[i] is where record i's string starts there (list_cap + 1 entries: the last one closes the pool)
-    unsigned long long *list_starts = nullptr;
-    char *lstr_pool = nullptr;
+    b200::DevBuf<unsigned long long> list_starts;
+    b200::DevBuf<char> lstr_pool;
     uint64_t lstr_pool_n = 0, lstr_pool_cap = 0;
     // after finish: int64 string offsets[list_total + 1], the gathered bytes, one validity byte per element
-    long long *lstr_off = nullptr;
-    char *lstr_bytes = nullptr;
-    uint8_t *lstr_valid = nullptr;
+    b200::DevBuf<long long> lstr_off;
+    b200::DevBuf<char> lstr_bytes;
+    b200::DevBuf<uint8_t> lstr_valid;
     uint64_t lstr_nbytes = 0;
+
+    ~b200_agg() {
+        if (chain)
+            cudaEventDestroy(chain);
+    }
 };
 
 namespace b200 {
@@ -177,9 +238,6 @@ struct Stager {
 };
 
 int slot_reserve(b200_ctx *ctx, Slot *s, size_t bytes);
-// grid cache of the context (api.cu): cudaMalloc on a miss; a released block must not be referenced by work in flight
-cudaError_t ctx_alloc(b200_ctx *ctx, void **out, size_t bytes);
-void ctx_release(b200_ctx *ctx, void *p, size_t bytes);
 bool is_device_pointer(const void *p);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }

@@ -502,8 +502,8 @@ extern "C" int b200_compact(b200_ctx *ctx, int slot, const uint8_t *keep, int nc
         p.out[c] = outs_device[c];
     }
     const uint8_t *d_keep = static_cast<const uint8_t *>(stg.dev(keep));
-    unsigned *d_counts = nullptr;
-    B200_CUDA(cudaMallocAsync(reinterpret_cast<void **>(&d_counts), (size_t)nblk * 4 + 16, sl->stream));
+    DevBuf<unsigned> d_counts;
+    B200_CHECK(d_counts.alloc(ctx, (size_t)nblk * 4 + 16, "b200_compact", sl->stream));
     unsigned long long *d_total = reinterpret_cast<unsigned long long *>(sl->dscratch);
     k_keep_count<<<nblk, kCompactBlock, 0, sl->stream>>>(d_keep, nrows, d_counts);
     k_scan_u32<<<1, 1024, 0, sl->stream>>>(d_counts, nblk, d_total);
@@ -512,7 +512,6 @@ extern "C" int b200_compact(b200_ctx *ctx, int slot, const uint8_t *keep, int nc
     B200_CUDA(cudaGetLastError());
     unsigned long long total = 0;
     B200_CUDA(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, sl->stream));
-    B200_CUDA(cudaFreeAsync(d_counts, sl->stream));
     B200_CUDA(cudaStreamSynchronize(sl->stream));
     *count_out = (int64_t)total;
     return B200_OK;

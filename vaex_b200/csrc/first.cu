@@ -178,13 +178,13 @@ int launch_first(b200_ctx *ctx, cudaStream_t stream, const FirstParams &p, bool 
     return B200_OK;
 }
 
-int launch_merge_first(cudaStream_t stream, b200_agg *dst, const b200_agg *src) {
+int launch_merge_first(cudaStream_t stream, b200_agg *dst, const FirstGrids &src) {
     uint64_t n = dst->cells;
     if (!n)
         return B200_OK;
     int blocks = (int)((n + 255) / 256 < kSmCount * 8 ? (n + 255) / 256 : kSmCount * 8);
-    k_merge_first<<<blocks, 256, 0, stream>>>(static_cast<unsigned long long *>(dst->state), static_cast<const unsigned long long *>(src->state), dst->grid,
-                                              src->grid, dst->order, src->order, dst->cell_masked, src->cell_masked, dtype_size(dst->dtype),
+    k_merge_first<<<blocks, 256, 0, stream>>>(static_cast<unsigned long long *>(dst->state.get()), static_cast<const unsigned long long *>(src.state), dst->grid,
+                                              src.grid, dst->order, src.order, dst->cell_masked, src.cell_masked, dtype_size(dst->dtype),
                                               dtype_size(dst->dtype2), n);
     B200_CUDA(cudaGetLastError());
     return B200_OK;

@@ -31,34 +31,33 @@ struct b200_set {
     b200_ctx *ctx = nullptr;
     int dtype = 0, nmaps = 1;
     int64_t limit = -1;
-    b200::SetSlot *table = nullptr; // insert table: first = tag
+    b200::DevBuf<b200::SetSlot> table; // insert table: first = tag
     uint64_t cap = 0;
-    unsigned long long *counts = nullptr; // counter<T> mode (src/hash_primitives.hpp:344-433): occurrences per slot, parallel to `table`
+    b200::DevBuf<unsigned long long> counts; // counter<T> mode (src/hash_primitives.hpp:344-433): occurrences per slot, parallel to `table`
     bool counting = false;
     bool hold_count_pass = false; // merge: keys are inserted first, the other set's counts are added afterwards
-    unsigned long long *d_ctr = nullptr; // see CTR_*
+    b200::DevBuf<unsigned long long> d_ctr; // see CTR_*
     int64_t seq = 0;
     bool dirty = true;
     // finalized view
-    b200::SetSlot *probe = nullptr; // first = global ordinal
+    b200::DevBuf<b200::SetSlot> probe; // first = global ordinal
     uint64_t probe_cap = 0;
-    long long *d_offsets = nullptr; // nmaps
-    std::vector<uint64_t> h_keys;   // canonical patterns in ordinal order (special slots hold 0); filled lazily from d_keys_ord
+    b200::DevBuf<long long> d_offsets; // nmaps
+    std::vector<uint64_t> h_keys;      // canonical patterns in ordinal order (special slots hold 0); filled lazily from d_keys_ord
     bool h_keys_valid = false;
-    unsigned long long *d_keys_ord = nullptr; // n_entries canonical patterns in ordinal order (device)
-    size_t keys_ord_bytes = 0, log_bytes = 0;  // sizes handed to ctx_alloc (the blocks go back to the context's cache)
-    uint64_t n_entries = 0;                   // keys + NaN + null slots
-    int64_t max_call_rows = 0;                // largest update so far: bounds the row part of every tag
+    b200::DevBuf<unsigned long long> d_keys_ord; // n_entries canonical patterns in ordinal order (device)
+    uint64_t n_entries = 0;                      // keys + NaN + null slots
+    int64_t max_call_rows = 0;                   // largest update so far: bounds the row part of every tag
     // string keys (ordered_set_string): the table's key is the reference's 64-bit string hash; the bytes of every distinct key live
     // in `pool`, described by `log` (one record per key, in claim order); slot_log[table slot] = index of the key's record
     bool strings = false;
-    char *pool = nullptr;
+    b200::DevBuf<char> pool;
     uint64_t pool_cap = 0;
-    b200::StrLog *log = nullptr;
-    unsigned *slot_log = nullptr;            // parallel to `table`
-    unsigned long long *d_strctr = nullptr;  // [0] records in `log`, [1] bytes used in `pool`
-    unsigned long long *d_str_off = nullptr; // finalized: pool offset of the key with ordinal i
-    unsigned *d_str_len = nullptr;
+    b200::DevBuf<b200::StrLog> log;
+    b200::DevBuf<unsigned> slot_log;           // parallel to `table`
+    b200::DevBuf<unsigned long long> d_strctr;  // [0] records in `log`, [1] bytes used in `pool`
+    b200::DevBuf<unsigned long long> d_str_off; // finalized: pool offset of the key with ordinal i
+    b200::DevBuf<unsigned> d_str_len;
     std::vector<int64_t> h_offsets;
     int64_t n_keys = 0, nan_count = 0, null_count = 0;
     int64_t nan_value = 0x7fffffff, null_value = 0x7fffffff; // src/hash_primitives.hpp:447
@@ -385,43 +384,39 @@ inline int nblocks(unsigned long long n, int threads = 256) {
     return (int)(b < kSmCount * 8ull ? (b ? b : 1) : kSmCount * 8ull);
 }
 
-// Tables, sort scratch and probe tables come from the context's block cache (ctx_alloc, api.cu): a groupby builds and drops a set per
-// key column and pass, and cudaMalloc / cudaFree synchronise the device and contend with the feeder threads' copies.
-int set_alloc_table(b200_set *s, uint64_t cap, cudaStream_t st) {
-    B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->table), cap * sizeof(SetSlot)));
-    s->cap = cap;
-    if (s->counting) {
-        B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->counts), cap * sizeof(unsigned long long)));
-        B200_CUDA(cudaMemsetAsync(s->counts, 0, cap * sizeof(unsigned long long), st));
-    }
-    if (s->strings)
-        B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->slot_log), cap * sizeof(unsigned)));
-    k_set_init<<<nblocks(cap), 256, 0, st>>>(s->table, cap);
-    B200_CUDA(cudaGetLastError());
-    return B200_OK;
-}
-
+// Tables, sort scratch and probe tables come from the context's block cache (DevBuf, common.cuh): a groupby builds and drops a set
+// per key column and pass, and cudaMalloc / cudaFree synchronise the device and contend with the feeder threads' copies.
+//
+// The table and its parallel arrays (counts, slot log, string log), built at `cap` slots and rehashed from the current ones.  The old
+// blocks go back to the cache once `st` has drained: every launch that touches a set's table, pool or logs runs under s->mu and its
+// stream is synchronised before the lock is released, so no other stream can still touch them.
 int set_grow(b200_set *s, cudaStream_t st, uint64_t new_cap = 0) {
-    SetSlot *old = s->table;
-    unsigned long long *old_counts = s->counts;
-    unsigned *old_slot_log = s->slot_log;
-    StrLog *old_log = s->log;
-    const size_t old_log_bytes = s->log_bytes;
-    uint64_t old_cap = s->cap;
-    B200_CHECK(set_alloc_table(s, new_cap > old_cap ? new_cap : old_cap * 4, st));
-    k_set_rehash<<<nblocks(old_cap), 256, 0, st>>>(old, old_cap, s->table, s->cap - 1, old_counts, s->counts, old_slot_log, s->slot_log);
-    B200_CUDA(cudaGetLastError());
-    if (s->strings) { // one record per key at most: the log is as long as the table
-        s->log_bytes = s->cap * sizeof(StrLog);
-        B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->log), s->log_bytes));
-        if (old_log)
-            B200_CUDA(cudaMemcpyAsync(s->log, old_log, old_cap * sizeof(StrLog), cudaMemcpyDeviceToDevice, st));
+    const uint64_t old_cap = s->cap, cap = new_cap > old_cap ? new_cap : old_cap * 4;
+    DevBuf<SetSlot> table;
+    DevBuf<unsigned long long> counts;
+    DevBuf<unsigned> slot_log;
+    DevBuf<StrLog> log;
+    B200_CHECK(table.alloc(s->ctx, cap * sizeof(SetSlot), "ordered_set table", st));
+    if (s->counting) {
+        B200_CHECK(counts.alloc(s->ctx, cap * sizeof(unsigned long long), "ordered_set table", st));
+        B200_CUDA(cudaMemsetAsync(counts, 0, cap * sizeof(unsigned long long), st));
     }
-    B200_CUDA(cudaStreamSynchronize(st)); // every launch that touches a set's table runs on (or is joined to) this stream
-    ctx_release(s->ctx, old, old_cap * sizeof(SetSlot));
-    ctx_release(s->ctx, old_counts, old_cap * sizeof(unsigned long long));
-    ctx_release(s->ctx, old_slot_log, old_cap * sizeof(unsigned));
-    ctx_release(s->ctx, old_log, old_log_bytes);
+    if (s->strings) { // one record per key at most: the log is as long as the table
+        B200_CHECK(slot_log.alloc(s->ctx, cap * sizeof(unsigned), "ordered_set table", st));
+        B200_CHECK(log.alloc(s->ctx, cap * sizeof(StrLog), "ordered_set table", st));
+    }
+    k_set_init<<<nblocks(cap), 256, 0, st>>>(table, cap);
+    B200_CUDA(cudaGetLastError());
+    if (old_cap) {
+        k_set_rehash<<<nblocks(old_cap), 256, 0, st>>>(s->table, old_cap, table, cap - 1, s->counts, counts, s->slot_log, slot_log);
+        B200_CUDA(cudaGetLastError());
+        if (s->strings)
+            B200_CUDA(cudaMemcpyAsync(log, s->log, old_cap * sizeof(StrLog), cudaMemcpyDeviceToDevice, st));
+        B200_CUDA(cudaStreamSynchronize(st));
+    }
+    table.unbind(), counts.unbind(), slot_log.unbind(), log.unbind();
+    s->table = std::move(table), s->counts = std::move(counts), s->slot_log = std::move(slot_log), s->log = std::move(log);
+    s->cap = cap;
     return B200_OK;
 }
 
@@ -463,10 +458,9 @@ int set_finalize(b200_set *s) {
     const unsigned nblk = radix_blocks(E);
     const size_t en = (size_t)(E ? E : 1);
     const size_t off_hist = 5 * en * 8, off_first = off_hist + align_up((size_t)256 * (nblk ? nblk : 1) * 4, 256), off_spec = off_first + align_up((size_t)s->nmaps * 8, 256);
-    char *work = nullptr;
-    const size_t work_bytes = off_spec + 256;
-    B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&work), work_bytes));
-    unsigned long long *ckey = reinterpret_cast<unsigned long long *>(work), *tagA = ckey + en, *valA = tagA + en, *tagB = valA + en, *valB = tagB + en;
+    DevBuf<char> work;
+    B200_CHECK(work.alloc(s->ctx, off_spec + 256, "set_finalize", st));
+    unsigned long long *ckey = reinterpret_cast<unsigned long long *>(work.get()), *tagA = ckey + en, *valA = tagA + en, *tagB = valA + en, *valB = tagB + en;
     unsigned *hist = reinterpret_cast<unsigned *>(work + off_hist);
     long long *d_first = reinterpret_cast<long long *>(work + off_first), *d_spec = reinterpret_cast<long long *>(work + off_spec);
     if (n_table)
@@ -526,17 +520,14 @@ int set_finalize(b200_set *s) {
     // probe table + keys in ordinal order
     // (every reader of the previous probe table / key array holds s->mu or ran on a stream that has been synchronised since)
     B200_CHECK(b200_ctx_sync(s->ctx, -1));
-    ctx_release(s->ctx, s->probe, s->probe_cap * sizeof(SetSlot));
-    s->probe = nullptr;
-    ctx_release(s->ctx, s->d_keys_ord, s->keys_ord_bytes);
-    s->d_keys_ord = nullptr;
+    s->probe.reset();
+    s->d_keys_ord.reset();
     uint64_t pc = 16;
     while (pc < 2 * (n_table + 1))
         pc <<= 1;
-    B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->probe), pc * sizeof(SetSlot)));
+    B200_CHECK(s->probe.alloc(s->ctx, pc * sizeof(SetSlot), "set_finalize"));
     s->probe_cap = pc;
-    s->keys_ord_bytes = en * 8;
-    B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->d_keys_ord), s->keys_ord_bytes));
+    B200_CHECK(s->d_keys_ord.alloc(s->ctx, en * 8, "set_finalize"));
     k_set_init<<<nblocks(pc), 256, 0, st>>>(s->probe, pc);
     B200_CUDA(cudaMemsetAsync(d_first, 0xff, (size_t)s->nmaps * 8, st)); // -1: shard without keys
     B200_CUDA(cudaMemsetAsync(d_spec, 0xff, 3 * 8, st));
@@ -548,7 +539,6 @@ int set_finalize(b200_set *s) {
     B200_CUDA(cudaMemcpyAsync(first.data(), d_first, (size_t)s->nmaps * 8, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaMemcpyAsync(spec, d_spec, sizeof spec, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    ctx_release(s->ctx, work, work_bytes);
 
     s->n_entries = E;
     s->h_keys.clear();
@@ -568,7 +558,7 @@ int set_finalize(b200_set *s) {
         s->h_offsets[m] = next;
     }
     if (!s->d_offsets)
-        B200_CUDA(cudaMalloc(&s->d_offsets, sizeof(long long) * s->nmaps));
+        B200_CHECK(s->d_offsets.alloc(s->ctx, sizeof(long long) * s->nmaps, "set_finalize"));
     B200_CUDA(cudaMemcpyAsync(s->d_offsets, s->h_offsets.data(), sizeof(long long) * s->nmaps, cudaMemcpyHostToDevice, st));
     B200_CUDA(cudaStreamSynchronize(st));
     s->dirty = false;
@@ -669,55 +659,38 @@ using namespace b200;
 
 extern "C" {
 
-int b200_set_create(b200_ctx *ctx, int dtype, int nmaps, int64_t limit, b200_set **out) {
+// ordered_set, counter (`counting`) and ordered_set_string (`strings`): a failure leaves nothing behind and *out untouched
+static int set_create(b200_ctx *ctx, int dtype, int nmaps, int64_t limit, bool counting, bool strings, b200_set **out) {
     if (!ctx || !out || dtype < 0 || dtype >= B200_NDTYPE || nmaps < 1 || nmaps > 32767) {
         set_error("b200_set_create: invalid argument");
         return B200_ERR_INVALID;
     }
     B200_CUDA(cudaSetDevice(ctx->device));
-    b200_set *s = new b200_set;
+    std::unique_ptr<b200_set, int (*)(b200_set *)> s(new b200_set, b200_set_destroy);
     s->ctx = ctx;
     s->dtype = dtype;
     s->nmaps = nmaps;
     s->limit = limit;
+    s->counting = counting;
+    s->strings = strings;
     cudaStream_t st = ctx->slots[0]->stream;
-    int rc = set_alloc_table(s, 1ull << 12, st);
-    if (rc) {
-        b200_set_destroy(s);
-        return rc;
-    }
+    B200_CHECK(set_grow(s.get(), st, 1ull << 12));
     unsigned long long init[CTR_N] = {0, 0, 0, 0, ~0ull, ~0ull, ~0ull, 0, 0, 0};
-    cudaError_t e = cudaMalloc(&s->d_ctr, sizeof(unsigned long long) * CTR_N);
-    if (e == cudaSuccess)
-        e = cudaMemcpyAsync(s->d_ctr, init, sizeof init, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess)
-        e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        b200_set_destroy(s); // the set and its table do not outlive a failed create
-        return cuda_fail(e, "b200_set_create: counters", __FILE__, __LINE__);
+    B200_CHECK(s->d_ctr.alloc(ctx, sizeof init, "b200_set_create"));
+    B200_CUDA(cudaMemcpyAsync(s->d_ctr, init, sizeof init, cudaMemcpyHostToDevice, st));
+    if (strings) {
+        B200_CHECK(s->d_strctr.alloc(ctx, 16, "b200_strset_create"));
+        B200_CUDA(cudaMemsetAsync(s->d_strctr, 0, 16, st));
     }
-    *out = s;
+    B200_CUDA(cudaStreamSynchronize(st));
+    *out = s.release();
     return B200_OK;
 }
 
+int b200_set_create(b200_ctx *ctx, int dtype, int nmaps, int64_t limit, b200_set **out) { return set_create(ctx, dtype, nmaps, limit, false, false, out); }
+
 // counter_<T>(nmaps) (src/hash_primitives.cpp:36-43): an ordered set that also counts the occurrences of every key
-int b200_counter_create(b200_ctx *ctx, int dtype, int nmaps, b200_set **out) {
-    B200_CHECK(b200_set_create(ctx, dtype, nmaps, -1, out));
-    b200_set *s = *out;
-    s->counting = true;
-    cudaStream_t st = ctx->slots[0]->stream;
-    cudaError_t e = ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->counts), s->cap * sizeof(unsigned long long));
-    if (e == cudaSuccess)
-        e = cudaMemsetAsync(s->counts, 0, s->cap * sizeof(unsigned long long), st);
-    if (e == cudaSuccess)
-        e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        b200_set_destroy(s);
-        *out = nullptr;
-        return cuda_fail(e, "b200_counter_create: counts", __FILE__, __LINE__);
-    }
-    return B200_OK;
-}
+int b200_counter_create(b200_ctx *ctx, int dtype, int nmaps, b200_set **out) { return set_create(ctx, dtype, nmaps, -1, true, false, out); }
 
 // counter::counts (src/hash_primitives.hpp:387-413) in the ordinal order of key_array(); the NaN / null slots hold their counts
 int b200_set_counts(b200_set *s, int64_t *out) {
@@ -732,15 +705,14 @@ int b200_set_counts(b200_set *s, int64_t *out) {
     const size_t n = (size_t)s->n_entries;
     if (!n)
         return B200_OK;
-    unsigned long long *d_out = nullptr;
-    B200_CUDA(cudaMalloc(&d_out, n * 8));
+    DevBuf<unsigned long long> d_out;
+    B200_CHECK(d_out.alloc(s->ctx, n * 8, "b200_set_counts", st));
     B200_CUDA(cudaMemsetAsync(d_out, 0, n * 8, st));
     k_counts_gather<<<nblocks(s->cap), 256, 0, st>>>(s->table, s->cap, s->counts, s->probe, s->probe_cap - 1, d_out);
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpyAsync(out, d_out, n * 8, cudaMemcpyDeviceToHost, st));
     unsigned long long h[CTR_N];
     B200_CHECK(read_ctr(s, st, h));
-    cudaFree(d_out);
     if (s->nan_count > 0)
         out[s->nan_value] = s->nan_count;
     if (s->null_count > 0)
@@ -756,18 +728,6 @@ int b200_set_destroy(b200_set *s) {
     cudaSetDevice(s->ctx->device);
     for (Slot *sl : s->ctx->slots) // the blocks go back to the cache: nothing in flight may still touch them
         cudaStreamSynchronize(sl->stream);
-    ctx_release(s->ctx, s->table, s->cap * sizeof(SetSlot));
-    ctx_release(s->ctx, s->counts, s->cap * sizeof(unsigned long long));
-    ctx_release(s->ctx, s->probe, s->probe_cap * sizeof(SetSlot));
-    ctx_release(s->ctx, s->d_keys_ord, s->keys_ord_bytes);
-    cudaFree(s->pool);
-    ctx_release(s->ctx, s->log, s->log_bytes);
-    ctx_release(s->ctx, s->slot_log, s->cap * sizeof(unsigned));
-    cudaFree(s->d_strctr);
-    cudaFree(s->d_str_off);
-    cudaFree(s->d_str_len);
-    cudaFree(s->d_ctr);
-    cudaFree(s->d_offsets);
     delete s;
     return B200_OK;
 }
@@ -802,18 +762,16 @@ int b200_set_update(b200_set *s, int slot, const void *keys, const uint8_t *mask
     B200_CHECK(set_insert_device(s, sl->stream, d_keys, d_masks, nrows, use_offsets, false, -1));
     if (return_values && nrows) {
         B200_CHECK(set_finalize(s));
-        long long *d_vals = nullptr;
-        short *d_map = nullptr;
-        B200_CUDA(cudaMalloc(&d_vals, sizeof(long long) * nrows));
-        B200_CUDA(cudaMalloc(&d_map, sizeof(short) * nrows));
+        DevBuf<long long> d_vals;
+        DevBuf<short> d_map;
+        B200_CHECK(d_vals.alloc(s->ctx, sizeof(long long) * nrows, "b200_set_update", sl->stream));
+        B200_CHECK(d_map.alloc(s->ctx, sizeof(short) * nrows, "b200_set_update", sl->stream));
         k_set_values<<<nblocks((unsigned long long)nrows), 256, 0, sl->stream>>>(s->probe, s->probe_cap - 1, s->sentinel_ordinal, s->nan_value, s->null_value,
                                                                                s->dtype, (int)isz, s->nmaps, s->d_offsets, d_keys, d_masks, nrows, d_vals, d_map);
         B200_CUDA(cudaGetLastError());
         B200_CUDA(cudaMemcpyAsync(out_values, d_vals, sizeof(long long) * nrows, cudaMemcpyDeviceToHost, sl->stream));
         B200_CUDA(cudaMemcpyAsync(out_map_index, d_map, sizeof(short) * nrows, cudaMemcpyDeviceToHost, sl->stream));
         B200_CUDA(cudaStreamSynchronize(sl->stream));
-        cudaFree(d_vals);
-        cudaFree(d_map);
     }
     (void)flags;
     return B200_OK;
@@ -1036,9 +994,12 @@ static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows
     stg.plan(keys, (size_t)nrows * isz);
     B200_CHECK(stg.commit());
     void *d_out = out;
+    DevBuf<> host_out;
     const bool out_host = memspace == B200_MEM_HOST || (memspace == B200_MEM_MIXED && !is_device_pointer(out));
-    if (out_host)
-        B200_CUDA(cudaMalloc(&d_out, nrows * osz));
+    if (out_host) {
+        B200_CHECK(host_out.alloc(s->ctx, nrows * osz, "b200_set_map", sl->stream));
+        d_out = host_out;
+    }
     k_set_map<<<nblocks((unsigned long long)nrows), 256, 0, sl->stream>>>(s->probe, s->probe_cap - 1, s->sentinel_ordinal,
                                                                         s->nan_count > 0 ? s->nan_value : -1, s->dtype, (int)isz, stg.dev(keys), nrows, d_out,
                                                                         out_isz);
@@ -1046,7 +1007,6 @@ static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows
     if (out_host) {
         B200_CUDA(cudaMemcpyAsync(out, d_out, nrows * osz, cudaMemcpyDeviceToHost, sl->stream));
         B200_CUDA(cudaStreamSynchronize(sl->stream));
-        cudaFree(d_out);
     }
     return B200_OK;
 }
@@ -1107,15 +1067,17 @@ int b200_set_combine(b200_ctx *ctx, int slot, int nkeys, b200_set *const *sets, 
         p.masks[k] = masks && masks[k] ? static_cast<const uint8_t *>(stg.dev(masks[k])) : nullptr;
     }
     long long *d_out = reinterpret_cast<long long *>(out);
+    DevBuf<long long> host_out;
     const bool out_host = memspace == B200_MEM_HOST || (memspace == B200_MEM_MIXED && !is_device_pointer(out));
-    if (out_host)
-        B200_CUDA(cudaMalloc(&d_out, nrows * 8));
+    if (out_host) {
+        B200_CHECK(host_out.alloc(ctx, nrows * 8, "b200_set_combine", sl->stream));
+        d_out = host_out;
+    }
     k_set_combine<<<nblocks((unsigned long long)nrows), 256, 0, sl->stream>>>(p, nrows, d_out);
     B200_CUDA(cudaGetLastError());
     if (out_host) {
         B200_CUDA(cudaMemcpyAsync(out, d_out, nrows * 8, cudaMemcpyDeviceToHost, sl->stream));
         B200_CUDA(cudaStreamSynchronize(sl->stream));
-        cudaFree(d_out);
     } else if (memspace != B200_MEM_DEVICE) {
         B200_CUDA(cudaStreamSynchronize(sl->stream)); // the caller's host key buffers are only valid during the call
     }
@@ -1329,13 +1291,10 @@ int str_finalize(b200_set *s) { // caller holds s->mu
     if (!was_dirty && s->d_str_off)
         return B200_OK;
     cudaStream_t st = s->ctx->slots[0]->stream;
-    if (s->d_str_off)
-        B200_CUDA(cudaFree(s->d_str_off));
-    if (s->d_str_len)
-        B200_CUDA(cudaFree(s->d_str_len));
+    // the previous index (if any) is replaced right after set_finalize synchronised every slot: nothing can still touch it
     const size_t en = (size_t)(s->n_entries ? s->n_entries : 1);
-    B200_CUDA(cudaMalloc(&s->d_str_off, en * 8));
-    B200_CUDA(cudaMalloc(&s->d_str_len, en * 4));
+    B200_CHECK(s->d_str_off.alloc(s->ctx, en * 8, "ordered_set_string"));
+    B200_CHECK(s->d_str_len.alloc(s->ctx, en * 4, "ordered_set_string"));
     B200_CUDA(cudaMemsetAsync(s->d_str_off, 0, en * 8, st));
     B200_CUDA(cudaMemsetAsync(s->d_str_len, 0, en * 4, st));
     unsigned long long sc[2];
@@ -1373,17 +1332,7 @@ int b200_strset_create(b200_ctx *ctx, int nmaps, int64_t limit, b200_set **out) 
         set_error("ordered_set_string: limit is not supported");
         return B200_ERR_UNSUPPORTED;
     }
-    B200_CHECK(b200_set_create(ctx, B200_U64, nmaps, -1, out));
-    b200_set *s = *out;
-    s->strings = true;
-    cudaStream_t st = ctx->slots[0]->stream;
-    B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->slot_log), s->cap * sizeof(unsigned)));
-    s->log_bytes = s->cap * sizeof(StrLog);
-    B200_CUDA(ctx_alloc(s->ctx, reinterpret_cast<void **>(&s->log), s->log_bytes));
-    B200_CUDA(cudaMalloc(&s->d_strctr, 16));
-    B200_CUDA(cudaMemsetAsync(s->d_strctr, 0, 16, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    return B200_OK;
+    return set_create(ctx, B200_U64, nmaps, -1, false, true, out);
 }
 
 int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, int return_values,
@@ -1417,16 +1366,16 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
         B200_CUDA(cudaMemcpyAsync(sc, s->d_strctr, 16, cudaMemcpyDeviceToHost, st));
         B200_CUDA(cudaStreamSynchronize(st));
         const uint64_t need = sc[1] + (uint64_t)in.nbytes + 16;
-        if (need > s->pool_cap) {
+        if (need > s->pool_cap) { // the old pool goes back once `st` has drained (see set_grow)
             const uint64_t cap = std::max<uint64_t>(need + need / 2, 1u << 20);
-            char *np = nullptr;
-            B200_CUDA(cudaMalloc(&np, cap));
+            DevBuf<char> np;
+            B200_CHECK(np.alloc(s->ctx, cap, "b200_strset_update", st));
             if (s->pool) {
                 B200_CUDA(cudaMemcpyAsync(np, s->pool, sc[1], cudaMemcpyDeviceToDevice, st));
                 B200_CUDA(cudaStreamSynchronize(st));
-                B200_CUDA(cudaFree(s->pool));
             }
-            s->pool = np;
+            np.unbind();
+            s->pool = std::move(np);
             s->pool_cap = cap;
         }
     }
@@ -1458,10 +1407,10 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
     B200_CHECK(str_check_error(s, st));
     if (return_values && nrows) {
         B200_CHECK(str_finalize(s));
-        long long *d_vals = nullptr;
-        short *d_map = nullptr;
-        B200_CUDA(cudaMalloc(&d_vals, sizeof(long long) * nrows));
-        B200_CUDA(cudaMalloc(&d_map, sizeof(short) * nrows));
+        DevBuf<long long> d_vals;
+        DevBuf<short> d_map;
+        B200_CHECK(d_vals.alloc(s->ctx, sizeof(long long) * nrows, "b200_strset_update", st));
+        B200_CHECK(d_map.alloc(s->ctx, sizeof(short) * nrows, "b200_strset_update", st));
         k_str_map<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->probe, s->probe_cap - 1, s->d_str_off, s->d_str_len, s->pool,
                                                                     s->null_count > 0 ? s->null_value : -1, s->nmaps, s->d_offsets, in.offsets, in.bytes, in.masks,
                                                                     in.base, nrows, d_vals, d_map, 1);
@@ -1469,8 +1418,6 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
         B200_CUDA(cudaMemcpyAsync(out_values, d_vals, sizeof(long long) * nrows, cudaMemcpyDeviceToHost, st));
         B200_CUDA(cudaMemcpyAsync(out_map_index, d_map, sizeof(short) * nrows, cudaMemcpyDeviceToHost, st));
         B200_CUDA(cudaStreamSynchronize(st));
-        cudaFree(d_vals);
-        cudaFree(d_map);
     }
     B200_CUDA(cudaStreamSynchronize(st)); // the caller's buffers are only valid during the call
     return B200_OK;
@@ -1495,17 +1442,18 @@ int b200_strset_map_ordinal(b200_set *s, int slot, const int64_t *offsets, const
     Stager stg{s->ctx, sl, memspace};
     StrInput in;
     B200_CHECK(stage_strings(sl, stg, offsets, bytes, masks, nrows, memspace, &in));
-    long long *d_out = out_is_device ? reinterpret_cast<long long *>(out) : nullptr;
-    if (!out_is_device)
-        B200_CUDA(cudaMalloc(&d_out, sizeof(long long) * nrows));
+    long long *d_out = reinterpret_cast<long long *>(out);
+    DevBuf<long long> host_out;
+    if (!out_is_device) {
+        B200_CHECK(host_out.alloc(s->ctx, sizeof(long long) * nrows, "b200_strset_map_ordinal", st));
+        d_out = host_out;
+    }
     k_str_map<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->probe, s->probe_cap - 1, s->d_str_off, s->d_str_len, s->pool, s->null_count > 0 ? s->null_value : -1,
                                                                 s->nmaps, s->d_offsets, in.offsets, in.bytes, in.masks, in.base, nrows, d_out, nullptr, 0);
     B200_CUDA(cudaGetLastError());
     if (!out_is_device)
         B200_CUDA(cudaMemcpyAsync(out, d_out, sizeof(long long) * nrows, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    if (!out_is_device)
-        cudaFree(d_out);
     return B200_OK;
 }
 
@@ -1554,17 +1502,15 @@ int b200_strset_key_array(b200_set *s, int64_t *offsets_out, uint8_t *bytes_out)
     if (!total || !bytes_out)
         return B200_OK;
     cudaStream_t st = s->ctx->slots[0]->stream;
-    unsigned *d_off = nullptr;
-    char *d_bytes = nullptr;
-    B200_CUDA(cudaMalloc(&d_off, (n + 1) * 4));
-    B200_CUDA(cudaMalloc(&d_bytes, total));
+    DevBuf<unsigned> d_off;
+    DevBuf<char> d_bytes;
+    B200_CHECK(d_off.alloc(s->ctx, (n + 1) * 4, "b200_strset_key_array", st));
+    B200_CHECK(d_bytes.alloc(s->ctx, total, "b200_strset_key_array", st));
     B200_CUDA(cudaMemcpyAsync(d_off, off.data(), (n + 1) * 4, cudaMemcpyHostToDevice, st));
     k_str_gather<<<nblocks(n), 256, 0, st>>>(s->d_str_off, s->d_str_len, d_off, s->pool, n, d_bytes);
     B200_CUDA(cudaGetLastError());
     B200_CUDA(cudaMemcpyAsync(bytes_out, d_bytes, total, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    cudaFree(d_off);
-    cudaFree(d_bytes);
     return B200_OK;
 }
 

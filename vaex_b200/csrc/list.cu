@@ -206,52 +206,52 @@ __global__ void __launch_bounds__(256) k_list_str_gather(const unsigned long lon
 
 } // namespace
 
-// room for `more` records (and, for strings, `more_bytes` pool bytes); caller holds a->nmu.  Growth synchronises the device: other
-// slots may be appending into the old arrays
-static int list_reserve(b200_agg *a, uint64_t more, uint64_t more_bytes) {
+// room for `more` records (and, for strings, `more_bytes` pool bytes); caller holds a->nmu.  Growth synchronises the device first:
+// every append into the old arrays was enqueued under a->nmu, on any slot, so once the device has drained and the copies on `st` have
+// finished, no stream can still touch the old blocks.
+static int list_reserve(b200_agg *a, cudaStream_t st, uint64_t more, uint64_t more_bytes) {
     const bool str = a->op == B200_AGG_LIST_STRING;
     if (a->list_n + more > a->list_cap) {
         B200_CUDA(cudaDeviceSynchronize());
         const uint64_t cap = std::max<uint64_t>((a->list_n + more) * 2, 1u << 16);
-        unsigned long long *nk = nullptr, *nv = nullptr, *ns = nullptr;
-        B200_CUDA(cudaMalloc(&nk, cap * 8));
-        B200_CUDA(cudaMalloc(&nv, cap * 8));
+        DevBuf<unsigned long long> nk, nv, ns;
+        B200_CHECK(nk.alloc(a->ctx, cap * 8, "AggList", st));
+        B200_CHECK(nv.alloc(a->ctx, cap * 8, "AggList", st));
         if (str)
-            B200_CUDA(cudaMalloc(&ns, (cap + 1) * 8));
+            B200_CHECK(ns.alloc(a->ctx, (cap + 1) * 8, "AggList", st));
         if (a->list_n) {
-            B200_CUDA(cudaMemcpy(nk, a->list_keys, a->list_n * 8, cudaMemcpyDeviceToDevice));
-            B200_CUDA(cudaMemcpy(nv, a->list_vals, a->list_n * 8, cudaMemcpyDeviceToDevice));
+            B200_CUDA(cudaMemcpyAsync(nk, a->list_keys, a->list_n * 8, cudaMemcpyDeviceToDevice, st));
+            B200_CUDA(cudaMemcpyAsync(nv, a->list_vals, a->list_n * 8, cudaMemcpyDeviceToDevice, st));
             if (str)
-                B200_CUDA(cudaMemcpy(ns, a->list_starts, a->list_n * 8, cudaMemcpyDeviceToDevice));
+                B200_CUDA(cudaMemcpyAsync(ns, a->list_starts, a->list_n * 8, cudaMemcpyDeviceToDevice, st));
+            B200_CUDA(cudaStreamSynchronize(st));
         }
-        cudaFree(a->list_keys);
-        cudaFree(a->list_vals);
-        cudaFree(a->list_starts);
-        a->list_keys = nk, a->list_vals = nv, a->list_starts = ns, a->list_cap = cap;
+        nk.unbind(), nv.unbind(), ns.unbind();
+        a->list_keys = std::move(nk), a->list_vals = std::move(nv), a->list_starts = std::move(ns), a->list_cap = cap;
     }
     if (str && (a->lstr_pool_n + more_bytes + 16 > a->lstr_pool_cap || !a->lstr_pool)) {
         B200_CUDA(cudaDeviceSynchronize());
         const uint64_t cap = std::max<uint64_t>((a->lstr_pool_n + more_bytes) * 2 + 16, 1u << 20); // + 16: the gather's read slack
-        char *np = nullptr;
-        B200_CUDA(cudaMalloc(&np, cap));
-        if (a->lstr_pool_n)
-            B200_CUDA(cudaMemcpy(np, a->lstr_pool, a->lstr_pool_n, cudaMemcpyDeviceToDevice));
-        cudaFree(a->lstr_pool);
-        a->lstr_pool = np, a->lstr_pool_cap = cap;
+        DevBuf<char> np;
+        B200_CHECK(np.alloc(a->ctx, cap, "AggList_string", st));
+        if (a->lstr_pool_n) {
+            B200_CUDA(cudaMemcpyAsync(np, a->lstr_pool, a->lstr_pool_n, cudaMemcpyDeviceToDevice, st));
+            B200_CUDA(cudaStreamSynchronize(st));
+        }
+        np.unbind();
+        a->lstr_pool = std::move(np), a->lstr_pool_cap = cap;
     }
     return B200_OK;
 }
 
-// one b200_bin call: reserve nrows records, append (api.cu calls this for B200_AGG_LIST aggregators)
+// one b200_bin call: reserve nrows records, append (api.cu calls this for B200_AGG_LIST aggregators).  The append is enqueued under
+// the aggregator's lock, like bin_list_string's.
 int bin_list(b200_ctx *ctx, Slot *sl, b200_agg *a, const DevBinner *db, int nbinners, const void *data, const uint8_t *mask, int64_t nrows, bool vec) {
-    unsigned long long base;
-    {
-        std::lock_guard<std::mutex> g(a->nmu);
-        B200_CHECK(list_reserve(a, (uint64_t)nrows, 0));
-        base = a->list_n;
-        a->list_n += (uint64_t)nrows;
-        a->list_sorted = false;
-    }
+    std::lock_guard<std::mutex> g(a->nmu);
+    B200_CHECK(list_reserve(a, sl->stream, (uint64_t)nrows, 0));
+    const unsigned long long base = a->list_n;
+    a->list_n += (uint64_t)nrows;
+    a->list_sorted = false;
     ListParams p;
     memset(&p, 0, sizeof p);
     p.nb = nbinners;
@@ -284,7 +284,7 @@ int bin_list(b200_ctx *ctx, Slot *sl, b200_agg *a, const DevBinner *db, int nbin
 // before it frees the old arrays) can never run between reading the pointers and using them.
 int bin_list_string(b200_ctx *ctx, Slot *sl, b200_agg *a, const DevBinner *db, int nbinners, const StrInput &in, int64_t nrows, bool vec) {
     std::lock_guard<std::mutex> g(a->nmu);
-    B200_CHECK(list_reserve(a, (uint64_t)nrows, (uint64_t)in.nbytes));
+    B200_CHECK(list_reserve(a, sl->stream, (uint64_t)nrows, (uint64_t)in.nbytes));
     ListStrParams p;
     memset(&p, 0, sizeof p);
     p.nb = nbinners;
@@ -326,11 +326,11 @@ static int list_sort_count(b200_agg *a, cudaStream_t st, unsigned long long maxk
             return B200_ERR_UNSUPPORTED;
         }
         const unsigned nblk = radix_blocks(n), tiles = radix_tiles(n);
-        unsigned long long *kb = nullptr, *vb = nullptr;
-        unsigned *hist = nullptr;
-        B200_CUDA(cudaMalloc(&kb, n * 8));
-        B200_CUDA(cudaMalloc(&vb, n * 8));
-        B200_CUDA(cudaMalloc(&hist, (size_t)256 * nblk * 4));
+        DevBuf<unsigned long long> kb, vb;
+        DevBuf<unsigned> hist;
+        B200_CHECK(kb.alloc(a->ctx, n * 8, "b200_agg_list_finish", st));
+        B200_CHECK(vb.alloc(a->ctx, n * 8, "b200_agg_list_finish", st));
+        B200_CHECK(hist.alloc(a->ctx, (size_t)256 * nblk * 4, "b200_agg_list_finish", st));
         unsigned long long *kin = a->list_keys, *vin = a->list_vals, *kout = kb, *vout = vb;
         for (int shift = 0; shift < 64 && (maxkey >> shift); shift += 8) {
             k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(kin, vin, n, shift, 0, hist, nblk, tiles);
@@ -340,44 +340,39 @@ static int list_sort_count(b200_agg *a, cudaStream_t st, unsigned long long maxk
             std::swap(kin, kout);
             std::swap(vin, vout);
         }
-        B200_CUDA(cudaStreamSynchronize(st));
         if (kin != a->list_keys) { // an odd number of passes: the sorted records sit in the scratch arrays, which have n entries
-            B200_CUDA(cudaMemcpy(a->list_keys, kin, n * 8, cudaMemcpyDeviceToDevice));
-            B200_CUDA(cudaMemcpy(a->list_vals, vin, n * 8, cudaMemcpyDeviceToDevice));
+            B200_CUDA(cudaMemcpyAsync(a->list_keys, kin, n * 8, cudaMemcpyDeviceToDevice, st));
+            B200_CUDA(cudaMemcpyAsync(a->list_vals, vin, n * 8, cudaMemcpyDeviceToDevice, st));
         }
-        cudaFree(kb);
-        cudaFree(vb);
-        cudaFree(hist);
+        B200_CUDA(cudaStreamSynchronize(st));
     }
     a->list_sorted = true;
     // per-cell counts -> offsets (kept on the device until read)
     const size_t cn = (size_t)a->cells + 1;
     if (!a->list_counts)
-        B200_CUDA(cudaMalloc((void **)&a->list_counts, cn * 4));
+        B200_CHECK(a->list_counts.alloc(a->ctx, cn * 4, "b200_agg_list_finish"));
     B200_CUDA(cudaMemsetAsync(a->list_counts, 0, cn * 4, st));
     if (n)
         k_list_count<<<nblocks_for(n), 256, 0, st>>>(a->list_keys, n, a->list_counts, a->cells, cell_shift);
-    unsigned long long *d_total = nullptr;
-    B200_CUDA(cudaMalloc((void **)&d_total, 8));
+    DevBuf<unsigned long long> d_total;
+    B200_CHECK(d_total.alloc(a->ctx, 8, "b200_agg_list_finish", st));
     k_scan_u32<<<1, 1024, 0, st>>>(a->list_counts, cn, d_total);
     B200_CUDA(cudaGetLastError());
     unsigned long long total = 0;
     B200_CUDA(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
-    cudaFree(d_total);
     a->list_total = total;
     return B200_OK;
 }
 
 // the string elements of the sorted records: int64 offsets (a scan of the lengths), the bytes gathered from the pool, validity
+// (the previous outputs are replaced under a->nmu with every slot synchronised, and their readers synchronise before they unlock)
 static int list_string_gather(b200_agg *a, cudaStream_t st) {
     const uint64_t total = a->list_total;
-    cudaFree(a->lstr_off);
-    cudaFree(a->lstr_bytes);
-    cudaFree(a->lstr_valid);
-    a->lstr_off = nullptr, a->lstr_bytes = nullptr, a->lstr_valid = nullptr, a->lstr_nbytes = 0;
-    B200_CUDA(cudaMalloc((void **)&a->lstr_off, (total + 1) * 8));
-    B200_CUDA(cudaMalloc((void **)&a->lstr_valid, total ? total : 1));
+    a->lstr_bytes.reset();
+    a->lstr_nbytes = 0;
+    B200_CHECK(a->lstr_off.alloc(a->ctx, (total + 1) * 8, "b200_agg_list_finish"));
+    B200_CHECK(a->lstr_valid.alloc(a->ctx, total, "b200_agg_list_finish"));
     B200_CUDA(cudaMemsetAsync(a->lstr_off + total, 0, 8, st));
     if (total) {
         // the record after the last one closes the pool
@@ -385,12 +380,15 @@ static int list_string_gather(b200_agg *a, cudaStream_t st) {
         k_list_str_len<<<nblocks_for(total), 256, 0, st>>>(a->list_vals, a->list_starts, total, a->lstr_off);
         B200_CUDA(cudaGetLastError());
     }
-    B200_CHECK(scan_i64(a->lstr_off, total + 1, st));
+    DevBuf<long long> tile_sums;
+    if (const unsigned long long ns = scan_i64_sums(total + 1))
+        B200_CHECK(tile_sums.alloc(a->ctx, ns * 8, "b200_agg_list_finish", st));
+    B200_CHECK(scan_i64(a->lstr_off, total + 1, tile_sums, st));
     long long nbytes = 0;
     B200_CUDA(cudaMemcpyAsync(&nbytes, a->lstr_off + total, 8, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
     a->lstr_nbytes = (uint64_t)nbytes;
-    B200_CUDA(cudaMalloc((void **)&a->lstr_bytes, a->lstr_nbytes ? a->lstr_nbytes : 1));
+    B200_CHECK(a->lstr_bytes.alloc(a->ctx, a->lstr_nbytes, "b200_agg_list_finish"));
     if (total) {
         // a group of threads per string, sized by the mean length: short strings must not leave most of a warp idle
         const uint64_t mean = a->lstr_nbytes / total;
@@ -447,15 +445,14 @@ int b200_agg_list_read(b200_agg *a, int64_t *offsets_out, void *values_out) {
     std::vector<unsigned> off(cn);
     B200_CUDA(cudaMemcpyAsync(off.data(), a->list_counts, cn * 4, cudaMemcpyDeviceToHost, st));
     const int isz = dtype_size(a->dtype);
-    void *d_out = nullptr;
+    DevBuf<> d_out;
     if (a->list_total && values_out) {
-        B200_CUDA(cudaMalloc(&d_out, a->list_total * isz));
+        B200_CHECK(d_out.alloc(a->ctx, a->list_total * isz, "b200_agg_list_read", st));
         k_list_values<<<nblocks_for(a->list_total), 256, 0, st>>>(a->list_keys, a->list_vals, a->list_total, a->dtype, isz, d_out);
         B200_CUDA(cudaGetLastError());
         B200_CUDA(cudaMemcpyAsync(values_out, d_out, a->list_total * isz, cudaMemcpyDeviceToHost, st));
     }
     B200_CUDA(cudaStreamSynchronize(st));
-    cudaFree(d_out);
     for (size_t i = 0; i < cn; i++)
         offsets_out[i] = (int64_t)off[i];
     return B200_OK;

@@ -221,27 +221,20 @@ int launch(b200_ctx *ctx, const MiArgs &a, cudaStream_t st) {
     }
     const int priv = (size_t)msum * sizeof(long long) + marg_static <= kMiSmemMax;
     const size_t marg_bytes = (size_t)a.cells * msum * 8, n_bytes = (size_t)a.cells * 8, part_bytes = (size_t)a.cells * chunks * 8;
-    char *scratch = nullptr;
-    B200_CUDA(ctx_alloc(ctx, (void **)&scratch, marg_bytes + n_bytes + part_bytes));
-    long long *gmarg = reinterpret_cast<long long *>(scratch), *gN = reinterpret_cast<long long *>(scratch + marg_bytes);
+    DevBuf<char> scratch;
+    B200_CHECK(scratch.alloc(ctx, marg_bytes + n_bytes + part_bytes, "b200_grid_mutual_information", st));
+    long long *gmarg = reinterpret_cast<long long *>(scratch.get()), *gN = reinterpret_cast<long long *>(scratch + marg_bytes);
     double *partial = reinterpret_cast<double *>(scratch + marg_bytes + n_bytes);
-    int rc = B200_OK;
-    cudaError_t e = cudaMemsetAsync(scratch, 0, marg_bytes + n_bytes, st);
-    if (e == cudaSuccess) {
-        const dim3 g((unsigned)chunks, (unsigned)std::min(a.cells, kMaxGridY));
-        k_mi_marg<<<g, kScanThreads, priv ? msum * sizeof(long long) : 0, st>>>(a, gmarg, gN, priv);
-        const long long norm_blocks = std::min<long long>((a.cells * msum + kScanThreads - 1) / kScanThreads, (long long)sm_count * 8);
-        k_mi_norm<<<(unsigned)norm_blocks, kScanThreads, 0, st>>>(a, gmarg, gN);
-        k_mi_terms<<<g, kScanThreads, 0, st>>>(a, reinterpret_cast<const double *>(gmarg), gN, partial, chunks);
-        k_mi_final<<<(unsigned)std::min(a.cells, kMaxGridY), kScanThreads, 0, st>>>(a, partial, chunks);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess)
-        e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess)
-        rc = cuda_fail(e, "k_mi_*", __FILE__, __LINE__);
-    ctx_release(ctx, scratch, marg_bytes + n_bytes + part_bytes);
-    return rc;
+    B200_CUDA(cudaMemsetAsync(scratch, 0, marg_bytes + n_bytes, st));
+    const dim3 g((unsigned)chunks, (unsigned)std::min(a.cells, kMaxGridY));
+    k_mi_marg<<<g, kScanThreads, priv ? msum * sizeof(long long) : 0, st>>>(a, gmarg, gN, priv);
+    const long long norm_blocks = std::min<long long>((a.cells * msum + kScanThreads - 1) / kScanThreads, (long long)sm_count * 8);
+    k_mi_norm<<<(unsigned)norm_blocks, kScanThreads, 0, st>>>(a, gmarg, gN);
+    k_mi_terms<<<g, kScanThreads, 0, st>>>(a, reinterpret_cast<const double *>(gmarg), gN, partial, chunks);
+    k_mi_final<<<(unsigned)std::min(a.cells, kMaxGridY), kScanThreads, 0, st>>>(a, partial, chunks);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaStreamSynchronize(st));
+    return B200_OK;
 }
 
 } // namespace
@@ -298,22 +291,15 @@ extern "C" int b200_grid_mutual_information(b200_ctx *ctx, int slot, const int64
     std::lock_guard<std::mutex> guard(sl->mu);
     cudaStream_t st = sl->stream;
     const size_t bytes = (size_t)a.cells * sizeof(double);
-    double *dout = out;
-    if (memspace_out == B200_MEM_HOST)
-        B200_CUDA(ctx_alloc(ctx, (void **)&dout, bytes));
-    a.out = dout;
-    int rc = launch(ctx, a, st);
+    DevBuf<double> host_out;
+    a.out = out;
     if (memspace_out == B200_MEM_HOST) {
-        if (rc == B200_OK) {
-            const cudaError_t e = cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, st);
-            if (e != cudaSuccess)
-                rc = cuda_fail(e, "cudaMemcpyAsync(out)", __FILE__, __LINE__);
-        }
+        B200_CHECK(host_out.alloc(ctx, bytes, "b200_grid_mutual_information", st));
+        a.out = host_out;
     }
-    const cudaError_t e = cudaStreamSynchronize(st);
-    if (rc == B200_OK && e != cudaSuccess)
-        rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+    B200_CHECK(launch(ctx, a, st));
     if (memspace_out == B200_MEM_HOST)
-        ctx_release(ctx, dout, bytes);
-    return rc;
+        B200_CUDA(cudaMemcpyAsync(out, host_out, bytes, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return B200_OK;
 }

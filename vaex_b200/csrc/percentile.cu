@@ -303,27 +303,22 @@ extern "C" int b200_grid_percentile(b200_ctx *ctx, int slot, const int64_t *grid
     cudaStream_t st = sl->stream;
     const size_t bytes = (size_t)a.cells * npct * sizeof(double);
     double *dout = out;
-    if (memspace_out == B200_MEM_HOST)
-        B200_CUDA(cudaMallocAsync((void **)&dout, bytes, st));
-    int rc = B200_OK;
-    for (int k0 = 0; k0 < npct && rc == B200_OK; k0 += kPctMax) {
+    DevBuf<double> host_out;
+    if (memspace_out == B200_MEM_HOST) {
+        B200_CHECK(host_out.alloc(ctx, bytes, "b200_grid_percentile", st));
+        dout = host_out;
+    }
+    for (int k0 = 0; k0 < npct; k0 += kPctMax) {
         a.npct = std::min(kPctMax, npct - k0);
         for (int k = 0; k < a.npct; k++) {
             a.pct[k] = pct[k0 + k];
             a.integral[k] = integral[k0 + k] != 0;
         }
         a.out = dout + (size_t)k0 * a.cells;
-        rc = launch(a, ctx->sm_count, st);
+        B200_CHECK(launch(a, ctx->sm_count, st));
     }
-    if (memspace_out == B200_MEM_HOST) {
-        if (rc == B200_OK) {
-            const cudaError_t e = cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, st);
-            if (e != cudaSuccess)
-                rc = cuda_fail(e, "cudaMemcpyAsync(out)", __FILE__, __LINE__);
-        }
-        cudaFreeAsync(dout, st);
-    }
-    B200_CHECK(rc);
+    if (memspace_out == B200_MEM_HOST)
+        B200_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
     return B200_OK;
 }

@@ -130,21 +130,26 @@ static __global__ void __launch_bounds__(kScanThreads) k_scan_i64_apply(long lon
     }
 }
 
-static inline int scan_i64(long long *a, unsigned long long n, cudaStream_t st) {
+// tile sums of every level of scan_i64(n): the caller provides them and keeps them until the scan has run
+static inline unsigned long long scan_i64_sums(unsigned long long n) {
+    unsigned long long total = 0;
+    for (; n > kScanTile; n = (n + kScanTile - 1) / kScanTile)
+        total += (n + kScanTile - 1) / kScanTile;
+    return total;
+}
+
+static inline int scan_i64(long long *a, unsigned long long n, long long *sums, cudaStream_t st) {
     if (n <= kScanTile) {
         k_scan_i64_apply<<<1, kScanThreads, 0, st>>>(a, n, nullptr);
         B200_CUDA(cudaGetLastError());
         return B200_OK;
     }
     const unsigned long long tiles = (n + kScanTile - 1) / kScanTile;
-    long long *sums = nullptr;
-    B200_CUDA(cudaMallocAsync((void **)&sums, tiles * 8, st));
     k_scan_i64_sums<<<(unsigned)tiles, kScanThreads, 0, st>>>(a, n, sums);
     B200_CUDA(cudaGetLastError());
-    B200_CHECK(scan_i64(sums, tiles, st));
+    B200_CHECK(scan_i64(sums, tiles, sums + tiles, st));
     k_scan_i64_apply<<<(unsigned)tiles, kScanThreads, 0, st>>>(a, n, sums);
     B200_CUDA(cudaGetLastError());
-    B200_CUDA(cudaFreeAsync(sums, st));
     return B200_OK;
 }
 

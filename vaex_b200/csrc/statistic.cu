@@ -545,10 +545,15 @@ struct b200_stat {
     double minv[B200_MAX_BINNERS] = {}, scale[B200_MAX_BINNERS] = {};
     long long stride[B200_MAX_BINNERS] = {};
     long long cells = 1;
-    unsigned long long *acc = nullptr;
+    DevBuf<unsigned long long> acc;
     size_t bytes = 0;
     cudaEvent_t chain = nullptr; // FIRST: select + deposit pairs of different slots must not interleave
     std::mutex chain_mu;
+
+    ~b200_stat() {
+        if (chain)
+            cudaEventDestroy(chain);
+    }
 };
 
 static int stat_fill(b200_stat *s, cudaStream_t st) {
@@ -577,18 +582,16 @@ int b200_stat_create(b200_ctx *ctx, int op, int cls, int ndim, const int64_t *si
         set_error("b200_stat_create: op %d needs %d weight(s), got %d", op, need, nweights);
         return B200_ERR_INVALID;
     }
-    b200_stat *s = new b200_stat;
+    std::unique_ptr<b200_stat, int (*)(b200_stat *)> s(new b200_stat, b200_stat_destroy);
     s->ctx = ctx, s->op = op, s->cls = cls, s->ndim = ndim, s->edges = edges != 0, s->nw = nweights, s->nsel = nselections;
     for (int d = ndim - 1; d >= 0; d--) { // C order: the first dimension is the slowest
         if (sizes[d] < 1 || sizes[d] > (1LL << 30) || (edges && sizes[d] < 3)) {
-            delete s;
             set_error("b200_stat_create: invalid size %lld of dimension %d", (long long)sizes[d], d);
             return B200_ERR_INVALID;
         }
         s->sizes[d] = sizes[d];
         s->stride[d] = s->cells;
         if (s->cells > (1LL << 40) / sizes[d]) {
-            delete s;
             set_error("b200_stat_create: grid too large");
             return B200_ERR_INVALID;
         }
@@ -615,27 +618,12 @@ int b200_stat_create(b200_ctx *ctx, int op, int cls, int ndim, const int64_t *si
     }
     s->bytes = (size_t)nselections * s->cells * s->K * 8;
     B200_CUDA(cudaSetDevice(ctx->device));
-    cudaError_t e = ctx_alloc(ctx, (void **)&s->acc, s->bytes);
-    if (e == cudaSuccess)
-        e = cudaEventCreateWithFlags(&s->chain, cudaEventDisableTiming);
-    if (e != cudaSuccess) {
-        b200_stat_destroy(s);
-        if (e == cudaErrorMemoryAllocation) {
-            cudaGetLastError();
-            set_error("b200_stat_create: out of device memory for %zu bytes", s->bytes);
-            return B200_ERR_NOMEM;
-        }
-        return cuda_fail(e, "cudaMalloc(stat)", __FILE__, __LINE__);
-    }
+    B200_CHECK(s->acc.alloc(ctx, s->bytes, "b200_stat_create"));
+    B200_CUDA(cudaEventCreateWithFlags(&s->chain, cudaEventDisableTiming));
     cudaStream_t st = ctx->slots[0]->stream;
-    int rc = stat_fill(s, st);
-    if (!rc && cudaStreamSynchronize(st) != cudaSuccess)
-        rc = B200_ERR_CUDA;
-    if (rc) {
-        b200_stat_destroy(s);
-        return rc;
-    }
-    *out = s;
+    B200_CHECK(stat_fill(s.get(), st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    *out = s.release();
     return B200_OK;
 }
 
@@ -645,10 +633,6 @@ int b200_stat_destroy(b200_stat *s) {
     cudaSetDevice(s->ctx->device);
     for (Slot *sl : s->ctx->slots)
         cudaStreamSynchronize(sl->stream);
-    if (s->acc)
-        ctx_release(s->ctx, s->acc, s->bytes);
-    if (s->chain)
-        cudaEventDestroy(s->chain);
     delete s;
     return B200_OK;
 }
