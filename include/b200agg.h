@@ -146,6 +146,10 @@ int b200_ctx_stream(b200_ctx *ctx, int slot, void **stream_out);
  * out[2] chunks reserved, out[3] entries per chunk, out[4] bytes memset before the batch, out[5] (warp, part) lists.
  * All zero when the slot has not run that path.  No reference counterpart (instrumentation). */
 int b200_ctx_path_stats(b200_ctx *ctx, int slot, uint64_t out[6]);
+/* Milliseconds of the last partitioned count(*) batch on this slot, from CUDA events that csrc/ringcount.cu records only while the
+ * environment variable B200_RING_EVENTS is 1 (read per call): out[0] the memset before the batch, out[1] k_ring_partition,
+ * out[2] k_ring_count.  Synchronises the slot's stream.  All zero when the last batch ran untimed.  No reference counterpart. */
+int b200_ctx_ring_times(b200_ctx *ctx, int slot, float out[3]);
 /* Wall-clock accounting of the host-chunk path (b200_bin with B200_MEM_HOST), summed over the slots: out[0..3] nanoseconds spent
  * waiting for a free piece of the page-locked bounce ring, in memcpy into the ring, enqueueing the pieces' copies, and in b200_bin
  * as a whole; out[4] pieces copied, out[5] calls.  reset != 0 zeroes the counters.  No reference counterpart (instrumentation). */

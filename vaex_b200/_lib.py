@@ -105,6 +105,7 @@ def lib():
             "b200_ctx_device": (i32, [vp]),
             "b200_ctx_stream": (i32, [vp, i32, P(vp)]),
             "b200_ctx_path_stats": (i32, [vp, i32, P(u64)]),
+            "b200_ctx_ring_times": (i32, [vp, i32, P(C.c_float)]),
             "b200_ctx_host_stats": (i32, [vp, P(u64), i32]),
             "b200_ctx_mem_stats": (i32, [vp, P(u64)]),
             "b200_ctx_occupy": (i32, [vp, i32, i32, i32, i32, u64]),
@@ -213,6 +214,13 @@ class Context:
         out = (C.c_uint64 * 6)()
         check(lib().b200_ctx_path_stats(self._h, int(slot), out))
         return dict(rows=out[0], entries=out[1], chunks=out[2], chunk_entries=out[3], memset_bytes=out[4], lists=out[5])
+
+    def ring_times(self, slot=0):
+        """Milliseconds of the last partitioned count(*) batch on this slot, recorded only while B200_RING_EVENTS=1 (include/b200agg.h
+        b200_ctx_ring_times): the memset before the batch, k_ring_partition, k_ring_count.  All zero when that batch ran untimed."""
+        out = (C.c_float * 3)()
+        check(lib().b200_ctx_ring_times(self._h, int(slot), out))
+        return dict(memset_ms=out[0], k1_ms=out[1], k2_ms=out[2])
 
     def host_stats(self, reset=False):
         """Where the host-chunk path spent its wall time (include/b200agg.h b200_ctx_host_stats), milliseconds summed over slots."""

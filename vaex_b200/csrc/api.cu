@@ -402,6 +402,9 @@ int b200_ctx_destroy(b200_ctx *ctx) {
         }
         if (s->h2d_done)
             cudaEventDestroy(s->h2d_done);
+        for (cudaEvent_t e : s->ring_ev)
+            if (e)
+                cudaEventDestroy(e);
         if (s->stream)
             cudaStreamDestroy(s->stream);
         delete s;
@@ -483,6 +486,22 @@ int b200_ctx_path_stats(b200_ctx *ctx, int slot, uint64_t out[6]) {
     for (unsigned v : len)
         entries += v;
     out[0] = s->ring_rows, out[1] = entries, out[2] = chunks, out[3] = s->ring_chunk_entries, out[4] = s->ring_memset_bytes, out[5] = s->ring_lists;
+    return B200_OK;
+}
+
+int b200_ctx_ring_times(b200_ctx *ctx, int slot, float out[3]) {
+    if (!ctx || slot < 0 || slot >= ctx->nslots || !out) {
+        set_error("b200_ctx_ring_times: invalid argument");
+        return B200_ERR_INVALID;
+    }
+    Slot *s = ctx->slots[slot];
+    out[0] = out[1] = out[2] = 0.f;
+    B200_CUDA(cudaSetDevice(ctx->device));
+    B200_CUDA(cudaStreamSynchronize(s->stream));
+    if (!s->ring_timed)
+        return B200_OK;
+    for (int i = 0; i < 3; i++)
+        B200_CUDA(cudaEventElapsedTime(out + i, s->ring_ev[i], s->ring_ev[i + 1]));
     return B200_OK;
 }
 

@@ -100,6 +100,9 @@ struct Slot {
     const unsigned *ring_len = nullptr, *ring_ctl = nullptr;
     size_t ring_lists = 0;
     uint64_t ring_rows = 0, ring_memset_bytes = 0, ring_chunk_entries = 0;
+    // B200_RING_EVENTS=1: events around the memset, K1 and K2 of the last ringcount batch (b200_ctx_ring_times); created on first use
+    cudaEvent_t ring_ev[4] = {};
+    bool ring_timed = false;
     std::mutex mu;
 };
 

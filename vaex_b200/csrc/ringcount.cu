@@ -3,11 +3,14 @@
 // Why two kernels: a direct kernel issues one RED per row, and the L2 retires only a fixed number of sector operations per clock
 // chip-wide, loads included, which caps the 2-D 1024^2 count far below the HBM stream rate.  Shared-memory atomics retire
 // several times more lanes per clock, but a 1027^2 grid is 4 MB even with 32-bit counters.  So the grid is
-// cut into <= 32 (else 64) GRID TILES ("parts") of <= 49152 consecutive cells and the rows are partitioned by part first:
+// cut into <= 32 (else 64) GRID TILES ("parts") of <= 49151 cells and the rows are partitioned by part first.  A part is every
+// 32nd (64th) row of the grid along the outermost key when ceil(rows / parts) grid rows fit one part (INTERLEAVED parts: a
+// crowded distribution spreads evenly over them), else a contiguous range of the index:
 //
 //   K1 k_ring_partition  every WARP is autonomous.  The keys of the NEXT 256-row group are loaded into registers (128-bit,
 //                        evict-first loads) while the current group is placed.
-//                        Per row: the bit-exact fp64 bin index, part = idx / tile_cells (one IMAD.HI), ONE shared-memory atomic
+//                        Per row: the bit-exact fp64 bin index, the part (outer cell mod parts, or idx / tile_cells by one
+//                        IMAD.HI), ONE shared-memory atomic
 //                        on the (warp, part) counter whose return value is the row's slot in that part's RING (96 entries), and
 //                        one 16-bit store of the local cell index into the ring.  Every 256 rows the rings that hold a full
 //                        LINE (64 entries = 128 bytes) append it to the part's current CHUNK in global memory — half a warp per
@@ -16,10 +19,11 @@
 //                        lanes instead would cost divergent 16-byte shared-memory accesses.)
 //                        Chunks (512..2048 entries) come from ONE pool: a warp reserves 32 chunks with one global atomic and
 //                        hands them to its parts with a ballot; the chunks of a (warp, part) form a linked list (next[]), its
-//                        head and entry count go to head[] / len[].  No per-part bucket provisioning, no overflow fallback, and
-//                        2 B/row of scratch whatever the distribution.
-//   K2 k_ring_count      one persistent CTA per SM takes a contiguous share of the (part, warp) lists (balanced by entry count:
-//                        every warp sees the same row distribution), keeps the part's u32 histogram in <= 192 KB of shared
+//                        head and entry count go to head[] / len[], every warp adds its entry counts to the part totals at exit.
+//                        No table is memset: K1 writes every entry of them K2 reads.  No per-part bucket provisioning, no
+//                        overflow fallback, and 2 B/row of scratch whatever the distribution.
+//   K2 k_ring_count      one persistent CTA per SM takes a contiguous share of the (part, warp) lists (balanced by entry count,
+//                        from K1's part totals: every warp sees the same row distribution), keeps the part's u32 histogram in <= 192 KB of shared
 //                        memory, walks the lists with 128-bit loads + one ATOMS per entry, and flushes the non-zero cells with one
 //                        RED.ADD.64 each when the part changes (1-2 flushes per CTA).
 //
@@ -41,20 +45,28 @@ struct RingParams : FloatKeys {
     float clamp_lo[3], clamp_hi[3]; // CLAMPED variant (fp32 keys): see bin_cell_m2_clamped
     long long row0, nrows;        // this batch
     unsigned cells;
-    unsigned tile_cells;          // cells per part (<= 49151): part = idx / tile_cells, local = idx % tile_cells < 2^16
+    unsigned tile_cells;          // cells per part (<= 49151): local cell index < tile_cells < 2^16; tile_cells is the pad entry
+    // contiguous parts: part = idx / tile_cells, local = idx % tile_cells
     unsigned neg_tile_cells;      // 2^32 - tile_cells: local = idx + part * neg_tile_cells in one IMAD
     unsigned magic;               // part == __umulhi(idx, magic) for every idx < cells (verified on the host)
+    // interleaved parts (`interleaved` != 0): with c the cell of the outermost key (the last one, stride outer_stride),
+    // part = c mod nparts_pad, local = (c / nparts_pad) * outer_stride + (idx - c * outer_stride)
+    int interleaved;
+    unsigned outer_stride;
+    unsigned inner_sum;           // stride_sum - outer_stride
+    unsigned part_shift;          // log2(nparts_pad)
     int nparts;
     int nparts_pad;               // 32 * PPL
     unsigned chunk_shift;         // chunk = 1 << chunk_shift entries (9..11)
     unsigned nchunks_cap;         // chunks in the pool
     unsigned nlists_w;            // warps of K1 (lists per part)
+    // Only the control block is memset; K1 writes every other table entry that K2 reads
     unsigned short *pool;         // chunk c = pool + (c << chunk_shift)
-    unsigned *next;               // per chunk: next chunk of the same (warp, part) list; kNone = last      (memset 0xFF)
-    unsigned short *unused;       // per chunk: entries at the tail that were never written                 (memset 0)
-    unsigned *head;               // [warp][nparts_pad]: first chunk of the list; kNone = empty               (memset 0xFF)
-    unsigned *len;                // [warp][nparts_pad]: entries in the list (pads included)                  (memset 0)
-    unsigned *ctl;                // [0] pool cursor in chunks                                                (memset 0)
+    unsigned *next;               // per chunk: next chunk of the same (warp, part) list; kNone = last   (set when the chunk opens)
+    unsigned short *unused;       // per chunk: entries at the tail that were never written              (0 when it opens)
+    unsigned *head;               // [warp][nparts_pad]: first chunk of the list; kNone = empty            (kNone at K1's start)
+    unsigned *len;                // [warp][nparts_pad]: entries in the list (pads included)               (at K1's exit)
+    unsigned *ctl;                // control block (memset 0): [0] pool cursor in chunks, [kPartTotals + part] entries of a part
     unsigned long long *grid;
 };
 
@@ -67,6 +79,8 @@ constexpr int kLineLanes = kLine / 8; // lanes that move one line with 16 bytes 
 constexpr unsigned kSuper = 32;   // chunks a warp reserves from the pool at a time
 constexpr unsigned kNone = 0xFFFFFFFFu;
 constexpr int kCountThreads = 1024;
+constexpr int kPartTotals = 64;   // ctl[kPartTotals + part]: entries of a part (pads included), summed by K1's warps
+constexpr size_t kCtlBytes = (kPartTotals + kRingParts) * 4;
 
 // CLAMPED index for fp32 keys: halves the load on the conversion pipe (F2F.F64.F32 + F2I.F64 per key on the quarter-rate XU
 // pipe).  The cell is a monotone function of the key (every step of
@@ -83,34 +97,61 @@ __device__ __forceinline__ int bin_cell_m2_clamped(float v, float lo, float hi, 
     return v != v ? -2 : i;
 }
 
-// one row: bit-exact index, part, ONE shared-memory atomic for the slot, one 16-bit store
-template <typename T, int ND, int RING, int RSTRIDE, bool CLAMPED>
+// cell - 2 (CLAMPED) or cell - 1 of key d: the index is the sum of these times the strides, plus 2 (or 1) x stride_sum
+template <typename T, bool CLAMPED>
+__device__ __forceinline__ int key_cell(const RingParams &p, T v, int d) {
+    if constexpr (CLAMPED)
+        return bin_cell_m2_clamped(v, p.clamp_lo[d], p.clamp_hi[d], p.vmin[d], p.scale[d], p.bins_d[d]);
+    else
+        return bin_cell_m1((double)v, p.vmin[d], p.scale[d], p.bins_d[d], p.bins[d]);
+}
+
+// one row: bit-exact index, part, ONE shared-memory atomic for the slot, one 16-bit store.
+// ILV: parts interleaved by the outermost key's cell (its value mod 32 * PPL) instead of contiguous ranges of the index: the rows
+// of a crowded distribution spread over all parts, so fewer lanes of a warp rank into the same counter at once.
+template <typename T, int ND, int RING, int RSTRIDE, bool CLAMPED, int PPL, bool ILV>
 __device__ __forceinline__ void place_row(const RingParams &p, const T (&v)[ND], unsigned *cnt, unsigned short *ring, unsigned &idx, unsigned &slot_out,
                                           unsigned &worst) {
-    unsigned id;
-    if constexpr (CLAMPED) {
-        id = 2 * p.stride_sum;
+    constexpr unsigned kBase = CLAMPED ? 2 : 1;
+    unsigned id, part, local;
+    if constexpr (ILV) {
+        constexpr unsigned kShift = PPL == 1 ? 5 : 6;
+        unsigned inner = kBase * p.inner_sum;
 #pragma unroll
-        for (int d = 0; d < ND; d++)
-            id += (unsigned)bin_cell_m2_clamped(v[d], p.clamp_lo[d], p.clamp_hi[d], p.vmin[d], p.scale[d], p.bins_d[d]) * p.stride[d];
+        for (int d = 0; d < ND - 1; d++)
+            inner += (unsigned)key_cell<T, CLAMPED>(p, v[d], d) * p.stride[d];
+        const unsigned c = (unsigned)key_cell<T, CLAMPED>(p, v[ND - 1], ND - 1) + kBase;
+        id = c * p.outer_stride + inner;
+        part = c & ((1u << kShift) - 1u);
+        local = (c >> kShift) * p.outer_stride + inner;
     } else {
-        id = p.stride_sum;
+        id = kBase * p.stride_sum;
 #pragma unroll
         for (int d = 0; d < ND; d++)
-            id += (unsigned)bin_cell_m1((double)v[d], p.vmin[d], p.scale[d], p.bins_d[d], p.bins[d]) * p.stride[d];
+            id += (unsigned)key_cell<T, CLAMPED>(p, v[d], d) * p.stride[d];
+        part = __umulhi(id, p.magic);
     }
     idx = id;
-    const unsigned part = __umulhi(id, p.magic);
     const unsigned slot = atomicAdd(cnt + part, 1u);
     slot_out = slot;
     worst = max(worst, slot);
+    if constexpr (!ILV)
+        local = id + part * p.neg_tile_cells; // after the atomic: one register less live across it
     if (slot < (unsigned)RING)
-        ring[part * RSTRIDE + slot] = (unsigned short)(id + part * p.neg_tile_cells);
+        ring[part * RSTRIDE + slot] = (unsigned short)local;
+}
+
+// the grid cell of entry `local` (< tile_cells) of `part`: one division for interleaved parts
+__device__ __forceinline__ unsigned long long grid_cell(const RingParams &p, unsigned part, unsigned local) {
+    if (!p.interleaved)
+        return (unsigned long long)part * p.tile_cells + local;
+    const unsigned q = local / p.outer_stride;
+    return (unsigned long long)((q << p.part_shift) | part) * p.outer_stride + (local - q * p.outer_stride);
 }
 
 // one group of 256 rows (8 per lane) whose keys the caller already holds in registers (loaded one group ahead).
 // Returns the largest slot a row of this lane was given (>= RING: that row did not fit, see `overflow`).
-template <typename T, int ND, int RING, int RSTRIDE, bool CLAMPED>
+template <typename T, int ND, int RING, int RSTRIDE, bool CLAMPED, int PPL, bool ILV>
 __device__ __forceinline__ unsigned group_rows_regs(const RingParams &p, const T (&c)[2][ND][4], unsigned *cnt, unsigned short *ring, unsigned idx[8],
                                                     unsigned slots[8]) {
     unsigned worst = 0;
@@ -122,13 +163,13 @@ __device__ __forceinline__ unsigned group_rows_regs(const RingParams &p, const T
 #pragma unroll
             for (int d = 0; d < ND; d++)
                 v[d] = c[q][d][j];
-            place_row<T, ND, RING, RSTRIDE, CLAMPED>(p, v, cnt, ring, idx[q * 4 + j], slots[q * 4 + j], worst);
+            place_row<T, ND, RING, RSTRIDE, CLAMPED, PPL, ILV>(p, v, cnt, ring, idx[q * 4 + j], slots[q * 4 + j], worst);
         }
     return worst;
 }
 
 // the ragged end of the batch: global loads with bounds; slots[] = kNone marks rows that do not exist
-template <typename T, int ND, int RING, int RSTRIDE, bool CLAMPED>
+template <typename T, int ND, int RING, int RSTRIDE, bool CLAMPED, int PPL, bool ILV>
 __device__ __forceinline__ unsigned group_rows_tail(const RingParams &p, long long gbase, long long tend, int lane, unsigned *cnt, unsigned short *ring,
                                                     unsigned idx[8], unsigned slots[8]) {
     unsigned worst = 0;
@@ -144,7 +185,7 @@ __device__ __forceinline__ unsigned group_rows_tail(const RingParams &p, long lo
 #pragma unroll
                 for (int d = 0; d < ND; d++)
                     v[d] = __ldcs(static_cast<const T *>(p.x[d]) + row);
-                place_row<T, ND, RING, RSTRIDE, CLAMPED>(p, v, cnt, ring, idx[q * 4 + j], slots[q * 4 + j], worst);
+                place_row<T, ND, RING, RSTRIDE, CLAMPED, PPL, ILV>(p, v, cnt, ring, idx[q * 4 + j], slots[q * 4 + j], worst);
             }
         }
     return worst;
@@ -174,7 +215,7 @@ struct Owner {
     unsigned total[PPL]; // entries written to this list so far
 };
 
-template <typename T, int ND, int PPL, int WARPS, bool CLAMPED>
+template <typename T, int ND, int PPL, int WARPS, bool CLAMPED, bool ILV>
 __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_constant__ RingParams p) {
     using L = RingLayout<PPL>;
     constexpr int RING = kRing, RSTRIDE = kRingStride;
@@ -193,6 +234,9 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
 
     const unsigned cshift = p.chunk_shift, csize = 1u << cshift;
     const long long wglobal = (long long)blockIdx.x * WARPS + warp, wtotal = (long long)gridDim.x * WARPS;
+#pragma unroll
+    for (int k = 0; k < PPL; k++) // empty lists until their first chunk opens (the owner lane overwrites its own entry)
+        p.head[(unsigned long long)wglobal * p.nparts_pad + lane + 32 * k] = kNone;
 
     Owner<PPL> own;
 #pragma unroll
@@ -244,6 +288,8 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
                         p.head[(unsigned long long)wglobal * p.nparts_pad + part] = newid;
                     else
                         p.next[own.cur[k]] = newid;
+                    p.next[newid] = kNone; // the list's last chunk until the next one opens; full until the final flush says otherwise
+                    p.unused[newid] = 0;
                     own.cur[k] = newid;
                     own.wpos[k] = newid << cshift;
                     own.wend[k] = own.wpos[k] + csize;
@@ -256,7 +302,7 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
                     for (unsigned e = 0; e < kLine; e++) {
                         const unsigned c = ring[part * RSTRIDE + e];
                         if (c < p.tile_cells)
-                            atomicAdd(p.grid + (unsigned long long)part * p.tile_cells + c, 1ull);
+                            atomicAdd(p.grid + grid_cell(p, part, c), 1ull);
                     }
                 }
                 cnt[part] = n - kLine;
@@ -307,7 +353,7 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
     };
     auto place = [&](const T (&c)[2][ND][4]) {
         unsigned idx[8], slots[8];
-        const unsigned worst = group_rows_regs<T, ND, RING, RSTRIDE, CLAMPED>(p, c, cnt, ring, idx, slots);
+        const unsigned worst = group_rows_regs<T, ND, RING, RSTRIDE, CLAMPED, PPL, ILV>(p, c, cnt, ring, idx, slots);
         __syncwarp();
         flush(false);
         if (__any_sync(0xffffffffu, worst >= (unsigned)RING))
@@ -335,23 +381,23 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
     // ---- the ragged end (< 256 rows), taken by the warp whose turn it is ------------------------------------------------------------
     if (ngroups * kGroupRows < p.nrows && ngroups % wtotal == wglobal) {
         unsigned idx[8], slots[8];
-        const unsigned worst = group_rows_tail<T, ND, RING, RSTRIDE, CLAMPED>(p, p.row0 + ngroups * kGroupRows, p.row0 + p.nrows, lane, cnt, ring, idx, slots);
+        const unsigned worst = group_rows_tail<T, ND, RING, RSTRIDE, CLAMPED, PPL, ILV>(p, p.row0 + ngroups * kGroupRows, p.row0 + p.nrows, lane, cnt, ring, idx, slots);
         __syncwarp();
         flush(false);
         if (__any_sync(0xffffffffu, worst >= (unsigned)RING))
             overflow(idx, slots);
         __syncwarp();
     }
-    // ---- the incomplete last lines, then the list descriptors ---------------------------------------------------------------
+    // ---- the incomplete last lines, then the list descriptors of every part (0 for the empty ones) and the part totals ---------
     flush(true);
 #pragma unroll
     for (int k = 0; k < PPL; k++) {
         const int part = lane + 32 * k;
-        if (part < p.nparts) {
-            if (own.cur[k] != kNone)
-                p.unused[own.cur[k]] = (unsigned short)(own.wend[k] - own.wpos[k]);
-            p.len[(unsigned long long)wglobal * p.nparts_pad + part] = own.total[k];
-        }
+        if (own.cur[k] != kNone)
+            p.unused[own.cur[k]] = (unsigned short)(own.wend[k] - own.wpos[k]);
+        p.len[(unsigned long long)wglobal * p.nparts_pad + part] = own.total[k];
+        if (own.total[k])
+            atomicAdd(p.ctl + kPartTotals + part, own.total[k]);
     }
 }
 
@@ -364,22 +410,20 @@ __global__ void __launch_bounds__(kCountThreads, 1) k_ring_count(const __grid_co
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nparts = p.nparts, npad = p.nparts_pad;
     const unsigned W = p.nlists_w;
-    // entries per part = sum over warps of len[w][part]
-    for (int part = warp; part < nparts; part += kCountThreads / 32) {
-        unsigned long long s = 0;
-        for (unsigned w = lane; w < W; w += 32)
-            s += p.len[(unsigned long long)w * npad + part];
+    // prefix over the part totals K1 left in the control block: one warp, lane l scans parts l and l + 32
+    if (warp == 0) {
+        unsigned long long a = lane < nparts ? p.ctl[kPartTotals + lane] : 0, b = lane + 32 < nparts ? p.ctl[kPartTotals + lane + 32] : 0;
 #pragma unroll
-        for (int o = 16; o; o >>= 1)
-            s += __shfl_xor_sync(0xffffffffu, s, o);
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long ua = __shfl_up_sync(0xffffffffu, a, o), ub = __shfl_up_sync(0xffffffffu, b, o);
+            if (lane >= o)
+                a += ua, b += ub;
+        }
+        b += __shfl_sync(0xffffffffu, a, 31);
+        s_part_entries[lane + 1] = a;
+        s_part_entries[lane + 33] = b;
         if (lane == 0)
-            s_part_entries[part + 1] = s;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        s_part_entries[0] = 0;
-        for (int i = 0; i < nparts; i++)
-            s_part_entries[i + 1] += s_part_entries[i];
+            s_part_entries[0] = 0;
     }
     __syncthreads();
     const unsigned long long total = s_part_entries[nparts];
@@ -433,11 +477,13 @@ __global__ void __launch_bounds__(kCountThreads, 1) k_ring_count(const __grid_co
             }
         }
         __syncthreads();
-        const unsigned long long cell0 = (unsigned long long)part * tc;
         for (int i = tid; i < (int)tc; i += kCountThreads) {
             const unsigned c = hist[i];
-            if (c && cell0 + i < p.cells)
-                atomicAdd(p.grid + cell0 + i, (unsigned long long)c);
+            if (c) {
+                const unsigned long long cell = grid_cell(p, (unsigned)part, (unsigned)i);
+                if (cell < p.cells)
+                    atomicAdd(p.grid + cell, (unsigned long long)c);
+            }
         }
         __syncthreads();
     }
@@ -456,7 +502,9 @@ int launch_partition(const FloatPlan &f, bool clamped, long long ctas, cudaStrea
         constexpr int ND = decltype(nd)::value;
         auto go = [&](auto ppl) -> int {
             constexpr int PPL = decltype(ppl)::value, WARPS = RingLayout<PPL>::kWarps;
-            auto kern = clamped ? k_ring_partition<T, ND, PPL, WARPS, std::is_same<T, float>::value> : k_ring_partition<T, ND, PPL, WARPS, false>;
+            constexpr bool kF32 = std::is_same<T, float>::value;
+            auto kern = p.interleaved ? (clamped ? k_ring_partition<T, ND, PPL, WARPS, kF32, true> : k_ring_partition<T, ND, PPL, WARPS, false, true>)
+                                      : (clamped ? k_ring_partition<T, ND, PPL, WARPS, kF32, false> : k_ring_partition<T, ND, PPL, WARPS, false, false>);
             constexpr size_t dyn = RingLayout<PPL>::kPerWarp * WARPS;
             B200_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
             kern<<<(int)ctas, WARPS * 32, dyn, st>>>(p);
@@ -554,10 +602,22 @@ int launch_ringcount(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken)
     bool clamped = f.xdtype == B200_F32;
     for (int i = 0; i < f.nd && clamped; i++)
         clamped = clamp_bounds(p.vmin[i], p.scale[i], p.bins_d[i], p.bins[i], &p.clamp_lo[i], &p.clamp_hi[i]);
-    // as few parts as possible (32, else 64): the ring memory of k_ring_partition scales with the parts per lane;
-    // tile_cells is nudged upwards until the one-instruction division is exact
+    // As few parts as possible (32, else 64): the ring memory of k_ring_partition scales with the parts per lane.  At either count,
+    // parts interleaved by the outermost key's cell when ceil(its cells / parts) rows of the grid fit one part: a crowded
+    // distribution then spreads over all parts instead of a few central ones, which both ranks the rows with fewer same-counter
+    // conflicts in k_ring_partition and gives k_ring_count parts of even size.  Otherwise (a huge inner dimension) contiguous
+    // ranges of the index, tile_cells nudged upwards until the one-instruction division is exact.
+    const unsigned long long outer_cells = (unsigned long long)p.bins[f.nd - 1] + 3, outer_stride = p.stride[f.nd - 1];
     unsigned tile_cells = 0, magic = 0;
-    for (int np = 32; np <= kRingParts && !tile_cells; np *= 2) {
+    int np = 32;
+    bool interleaved = false;
+    for (; np <= kRingParts && !tile_cells; np *= 2) {
+        const unsigned long long ilv_cells = (outer_cells + np - 1) / np * outer_stride;
+        if (outer_cells * outer_stride == cells && ilv_cells <= kRingTileCells) {
+            tile_cells = (unsigned)ilv_cells;
+            interleaved = true;
+            break;
+        }
         unsigned long long tcells = ((cells + np - 1) / np + 7) / 8 * 8;
         for (int tries = 0; tries < 64 && tcells <= kRingTileCells; tries++, tcells += 8) {
             const unsigned m = (unsigned)((1ull << 32) / tcells) + 1u;
@@ -567,15 +627,26 @@ int launch_ringcount(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken)
                 break;
             }
         }
+        if (tile_cells)
+            break;
     }
     if (!tile_cells)
         return B200_OK;
     p.cells = (unsigned)cells;
     p.tile_cells = tile_cells;
-    p.neg_tile_cells = 0u - tile_cells;
-    p.magic = magic;
-    p.nparts = (int)((cells + tile_cells - 1) / tile_cells);
-    p.nparts_pad = p.nparts <= 32 ? 32 : 64;
+    if (interleaved) {
+        p.interleaved = 1;
+        p.outer_stride = (unsigned)outer_stride;
+        p.inner_sum = p.stride_sum - p.outer_stride;
+        p.nparts = (int)std::min<unsigned long long>(np, outer_cells);
+        p.nparts_pad = np;
+        p.part_shift = np == 32 ? 5 : 6;
+    } else {
+        p.neg_tile_cells = 0u - tile_cells;
+        p.magic = magic;
+        p.nparts = (int)((cells + tile_cells - 1) / tile_cells);
+        p.nparts_pad = p.nparts <= 32 ? 32 : 64;
+    }
     p.grid = f.p.count_star;
 
     // batches of <= 2^30 rows (32-bit entry counts), EQUAL in size: a 2^30 + remainder split paid the fixed cost of a pass (memsets,
@@ -596,10 +667,10 @@ int launch_ringcount(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken)
         return B200_OK;
     p.nchunks_cap = (unsigned)nchunks;
     const size_t lists = (size_t)nwarps * p.nparts_pad;
-    // layout: [ctl 256 B | len | unused] (zeroed)  [head | next] (0xFF)  [pool]
-    const size_t off_len = 256, off_unused = align_up(off_len + lists * 4, 256), zero_end = align_up(off_unused + nchunks * 2, 256);
-    const size_t off_head = zero_end, off_next = align_up(off_head + lists * 4, 256), ff_end = align_up(off_next + nchunks * 4, 256);
-    const size_t off_pool = ff_end;
+    // layout: [ctl] (zeroed before every batch)  [len | unused | head | next] (written by k_ring_partition)  [pool]
+    const size_t zero_end = align_up(kCtlBytes, 256), off_len = zero_end, off_unused = align_up(off_len + lists * 4, 256);
+    const size_t off_head = align_up(off_unused + nchunks * 2, 256), off_next = align_up(off_head + lists * 4, 256);
+    const size_t off_pool = align_up(off_next + nchunks * 4, 256);
     bool room = false;
     B200_CHECK(slot_scratch(slot, off_pool + (nchunks << cshift) * 2, &room));
     if (!room) // not enough memory for the pool: the direct RED kernel takes the call
@@ -614,19 +685,32 @@ int launch_ringcount(b200_ctx *ctx, Slot *slot, const FloatPlan &f, bool *taken)
     cudaStream_t st = slot->stream;
     B200_CUDA(cudaFuncSetAttribute(k_ring_count, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((kRingTileCells + 1) * 4)));
     const size_t hist_bytes = ((size_t)tile_cells / 4 + 1) * 16;
+    // B200_RING_EVENTS=1: events around the memsets, K1 and K2 of every batch; b200_ctx_ring_times reads those of the last one
+    const bool timed = env_ll("B200_RING_EVENTS", 0) == 1;
+    if (timed && !slot->ring_ev[0])
+        for (cudaEvent_t &e : slot->ring_ev)
+            B200_CUDA(cudaEventCreate(&e));
+    slot->ring_timed = timed;
     for (long long r0 = 0; r0 < nrows; r0 += batch) {
         p.row0 = r0;
         p.nrows = std::min<long long>(batch, nrows - r0);
+        if (timed)
+            B200_CUDA(cudaEventRecord(slot->ring_ev[0], st));
         B200_CUDA(cudaMemsetAsync(base, 0, zero_end, st));
-        B200_CUDA(cudaMemsetAsync(base + off_head, 0xFF, ff_end - off_head, st));
+        if (timed)
+            B200_CUDA(cudaEventRecord(slot->ring_ev[1], st));
         const long long ctas = partition_ctas(p.nrows, warps, ctx->sm_count);
         B200_CHECK(launch_partition(f, clamped, ctas, st, p));
+        if (timed)
+            B200_CUDA(cudaEventRecord(slot->ring_ev[2], st));
         const long long w = ctas * warps;
         p.nlists_w = (unsigned)w; // the last batch may launch fewer warps; its lists are the first w rows of head[] / len[]
         k_ring_count<<<ctx->sm_count, kCountThreads, hist_bytes, st>>>(p);
         B200_CUDA(cudaGetLastError());
+        if (timed)
+            B200_CUDA(cudaEventRecord(slot->ring_ev[3], st));
         slot->ring_len = p.len, slot->ring_ctl = p.ctl, slot->ring_lists = (size_t)w * p.nparts_pad;
-        slot->ring_rows = (uint64_t)p.nrows, slot->ring_memset_bytes = zero_end + (ff_end - off_head), slot->ring_chunk_entries = 1u << cshift;
+        slot->ring_rows = (uint64_t)p.nrows, slot->ring_memset_bytes = zero_end, slot->ring_chunk_entries = 1u << cshift;
     }
     *taken = true;
     return B200_OK;
