@@ -94,11 +94,13 @@ typedef enum {
    host columns are staged, device columns are used in place — e.g. device-computed group codes next to host value columns */
 typedef enum { B200_MEM_HOST = 0, B200_MEM_DEVICE = 1, B200_MEM_MIXED = 2 } b200_memspace;
 
-/* flags for b200_bin / b200_set_update */
+/* flags for b200_bin / b200_stat_bin / b200_set_update / b200_set_map_ordinal / b200_set_isin */
 /* Host chunks (B200_MEM_HOST) are by default memcpy'd into the slot's page-locked bounce ring inside the call: the caller's buffers
- * are only read during the call (vaex/cpu.py:708-710) and the call returns without waiting for the device.  With
- * B200_FLAG_ASYNC_HOST the copies are issued straight from the caller's buffers, which must then stay valid (and should be
- * page-locked, b200_host_register) until b200_ctx_sync(slot). */
+ * are only read during the call (vaex/cpu.py:708-710) and the call returns without waiting for the device.  The host columns of a
+ * MIXED call are copied straight from the caller's buffers, so the call waits for its stream before it returns.  With
+ * B200_FLAG_ASYNC_HOST the copies are issued straight from the caller's buffers in both cases and neither waits: the buffers must
+ * then stay valid (and should be page-locked, b200_host_register) until b200_ctx_sync(slot).  A call whose result goes to host
+ * memory always waits for it. */
 #define B200_FLAG_ASYNC_HOST 1u
 
 typedef struct b200_ctx b200_ctx;
@@ -150,9 +152,9 @@ int b200_ctx_path_stats(b200_ctx *ctx, int slot, uint64_t out[6]);
  * environment variable B200_RING_EVENTS is 1 (read per call): out[0] the memset before the batch, out[1] k_ring_partition,
  * out[2] k_ring_count.  Synchronises the slot's stream.  All zero when the last batch ran untimed.  No reference counterpart. */
 int b200_ctx_ring_times(b200_ctx *ctx, int slot, float out[3]);
-/* Wall-clock accounting of the host-chunk path (b200_bin with B200_MEM_HOST), summed over the slots: out[0..3] nanoseconds spent
- * waiting for a free piece of the page-locked bounce ring, in memcpy into the ring, enqueueing the pieces' copies, and in b200_bin
- * as a whole; out[4] pieces copied, out[5] calls.  reset != 0 zeroes the counters.  No reference counterpart (instrumentation). */
+/* Wall-clock accounting of the host-chunk path (the per-slot calls with B200_MEM_HOST), summed over the slots: out[0..3] nanoseconds
+ * spent waiting for a free piece of the page-locked bounce ring, in memcpy into the ring, enqueueing the pieces' copies, and in the
+ * calls as a whole; out[4] pieces copied, out[5] calls.  reset != 0 zeroes the counters.  No reference counterpart (instrumentation). */
 int b200_ctx_host_stats(b200_ctx *ctx, uint64_t out[6], int reset);
 /* Device memory of the context's block cache, in bytes: out[0] handed out and not yet returned (grids, sets, statistics and per-call
  * temporaries; the slots' staging and partition arenas are not counted), out[1] held idle in the cache.  No reference counterpart. */
@@ -233,13 +235,16 @@ int b200_set_offsets(b200_set *set, int64_t *out /* nmaps */);
 int b200_set_key_array(b200_set *set, void *keys_out /* count * itemsize, host */);
 /* out dtype follows the reference: count < 2^7 -> I8, < 2^15 -> I16, < 2^31 -> I32, else I64 */
 int b200_set_ordinal_dtype(b200_set *set);
+/* out: nrows ordinals / isin bytes, in device memory in a B200_MEM_DEVICE call, otherwise in host or device memory (classified
+   with cudaPointerGetAttributes) */
 int b200_set_map_ordinal(b200_set *set, int slot, const void *keys, int64_t nrows, void *out, int memspace, uint32_t flags);
 int b200_set_isin(b200_set *set, int slot, const void *keys, int64_t nrows, uint8_t *out, int memspace, uint32_t flags);
 size_t b200_set_bytes(b200_set *set);
 /* Sparse multi-key groupby (vaex/groupby.py:526-584 `_combine`: `sum_k _ordinal_values(key_k) * cumulative_counts[k+1]`,
    vaex/functions.py:2454-2463): per row, the ordinal of every key column in its own set (null rows -> the set's null ordinal,
    NaN -> its NaN ordinal) fused into ONE int64 code = sum_k ordinal_k * multipliers[k]; -1 when a key is in none of the
-   sets.  `masks[k]` may be NULL; `out` holds nrows int64 in the call's memspace. */
+   sets.  `masks[k]` may be NULL; `out` holds nrows int64 in device memory in a B200_MEM_DEVICE call, otherwise in host or device
+   memory (classified with cudaPointerGetAttributes). */
 #define B200_MAX_COMBINE 8
 int b200_set_combine(b200_ctx *ctx, int slot, int nkeys, b200_set *const *sets, const void *const *keys, const uint8_t *const *masks,
                      const int64_t *multipliers, int64_t nrows, int64_t *out, int memspace, uint32_t flags);

@@ -5,14 +5,21 @@ builds a problem that selects one variant, records the kernels the call launched
 is among them, and compares the grids with the oracle bit for bit, or with exact arithmetic where DESIGN §3 says bits cannot
 match (helpers.check_exact).  A threshold that moves makes these tests fail instead of silently moving coverage.
 """
+import json
+import os
 import re
+import subprocess
+import sys
 from fractions import Fraction
 
 import numpy as np
 import pytest
 
-import golden_util
-from helpers import B200Binby, check_exact, edge_column, gamma, random_case, same_bits
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path[:0] = [HERE, os.path.dirname(HERE)]
+
+import golden_util  # noqa: E402
+from helpers import B200Binby, check_exact, edge_column, gamma, random_case, same_bits  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -231,45 +238,87 @@ def test_nunique_table_grows_between_calls():
 
 
 # ---- heavy cells ---------------------------------------------------------------------------------------------------------------
-def test_heavy_cells_through_both_smem_kernels():
+HEAVY_N = 100_000_000
+
+
+def _heavy_columns():
+    import torch
+    i = torch.arange(HEAVY_N, device="cuda", dtype=torch.int64)
+    r = i % 1024
+    canc = torch.where(i % 2 == 0, 1e8, -1e8).to(torch.float64) + r.to(torch.float64) / 1024  # exact in float64
+    small = ((i % 7) - 3).to(torch.float32)
+    return i, r, canc, small
+
+
+def _heavy_grid(i, C, fast):
+    """(cell of every row, binner, grid): 13 float-key cells for fast.cu, 16 ordinal cells for k_binby"""
+    import torch
+    from vaex_b200 import superagg
+    cell = i % C
+    if fast:
+        bx = superagg.BinnerScalar_float32(1, "x", 0, C, C)
+        bx.set_data(0, cell.to(torch.float32) + 0.5)
+    else:
+        bx = superagg.BinnerOrdinal_int32(1, "x", C, 0, False, False)
+        bx.set_data(0, cell.to(torch.int32))
+    return cell, bx, superagg.Grid([bx])
+
+
+def _heavy_specs(fast, i, canc, small):
+    if fast:
+        return [("AggCount_int64", None), ("AggCount_float32", small), ("AggSum_float32", small), ("AggSumMoment_float32", small)]
+    return [("AggCount_int64", None), ("AggSum_float64", canc), ("AggSum_int64", i), ("AggMax_float64", canc)]
+
+
+def _heavy_bin(grid, specs):
+    from vaex_b200 import superagg
+    aggs = []
+    for cls, col in specs:
+        a = getattr(superagg, cls)(grid, 1, 1, 2) if "Moment" in cls else getattr(superagg, cls)(grid, 1, 1)
+        if col is not None:
+            a.set_data(0, col, 0)
+        a.clear_data_mask(0)
+        aggs.append(a)
+    grid.bin(0, aggs, HEAVY_N)
+    return [a.get_result() for a in aggs]
+
+
+def _record_fresh_kernels(path):
+    """the kernels of the heavy-cells binnings and of the count past 2^32"""
+    i, r, canc, small = _heavy_columns()
+    out = {}
+    for C, fast in ((13, True), (16, False)):
+        cell, bx, grid = _heavy_grid(i, C, fast)
+        out[str(C)] = sorted(launched(lambda: _heavy_bin(grid, _heavy_specs(fast, i, canc, small)))[1])
+        if fast:
+            out["13_f64"] = sorted(launched(lambda: _heavy_bin(grid, [("AggSum_float64", canc)]))[1])
+    del i, r, canc, small, cell, bx, grid
+    out["count_2p32"] = sorted(launched(_count_past_2p32)[1])
+    with open(path, "w") as fh:
+        json.dump(out, fh)
+
+
+@pytest.fixture(scope="module")
+def fresh_kernels(tmp_path_factory):
+    """the kernels the heavy-cells binnings and the count past 2^32 launched, recorded with torch.profiler in a fresh process: late in a long pytest process
+    the profiler's sessions come back without kernel records more and more often"""
+    out = tmp_path_factory.mktemp("prof") / "kernels.json"
+    subprocess.check_call([sys.executable, os.path.abspath(__file__), str(out)], cwd=os.path.dirname(HERE))
+    return json.loads(out.read_text())
+
+
+def test_heavy_cells_through_both_smem_kernels(fresh_kernels):
     """1e8 rows into 13 (fast.cu) and 16 (k_binby) cells: the private shared-memory sums and their flush.  Integer-valued floats
     sum exactly, so those sums are bit-exact; a cancelling column (+-1e8 plus dyadic residuals) is held to the recursive-summation
     bound of its exact sum; integer sums and counts are exact."""
     import torch
-    from vaex_b200 import superagg
-    n = 100_000_000
-    i = torch.arange(n, device="cuda", dtype=torch.int64)
-    r = i % 1024
-    canc = torch.where(i % 2 == 0, 1e8, -1e8).to(torch.float64) + r.to(torch.float64) / 1024  # exact in float64
-    small = ((i % 7) - 3).to(torch.float32)
+    i, r, canc, small = _heavy_columns()
     for C, fast in ((13, True), (16, False)):
-        cell = i % C
-        if fast:
-            bx = superagg.BinnerScalar_float32(1, "x", 0, C, C)
-            bx.set_data(0, cell.to(torch.float32) + 0.5)
-        else:
-            bx = superagg.BinnerOrdinal_int32(1, "x", C, 0, False, False)
-            bx.set_data(0, cell.to(torch.int32))
-        grid = superagg.Grid([bx])
-        if fast:
-            specs = [("AggCount_int64", None), ("AggCount_float32", small), ("AggSum_float32", small), ("AggSumMoment_float32", small)]
-        else:
-            specs = [("AggCount_int64", None), ("AggSum_float64", canc), ("AggSum_int64", i), ("AggMax_float64", canc)]
-
-        def go(specs=specs, grid=grid):
-            aggs = []
-            for cls, col in specs:
-                a = getattr(superagg, cls)(grid, 1, 1, 2) if "Moment" in cls else getattr(superagg, cls)(grid, 1, 1)
-                if col is not None:
-                    a.set_data(0, col, 0)
-                a.clear_data_mask(0)
-                aggs.append(a)
-            grid.bin(0, aggs, n)
-            return [a.get_result() for a in aggs]
-        got, names = launched(go)
+        cell, bx, grid = _heavy_grid(i, C, fast)
+        got, names = _heavy_bin(grid, _heavy_specs(fast, i, canc, small)), fresh_kernels[str(C)]
         inner = slice(2, C + 2) if fast else slice(0, C)
         counts = torch.bincount(cell, minlength=C).cpu().numpy()
-        assert got[0][inner].tolist() == counts.tolist() and got[0].sum() == n
+        assert got[0][inner].tolist() == counts.tolist() and got[0].sum() == HEAVY_N
         if fast:
             assert_ran(names, r"k_binby_fast<float, 1, float, true, true>")
             s = small.double()
@@ -277,7 +326,7 @@ def test_heavy_cells_through_both_smem_kernels():
             assert got[2][inner].tolist() == torch.zeros(C, dtype=torch.float64, device="cuda").index_add_(0, cell, s).cpu().tolist()
             assert got[3][inner].tolist() == torch.zeros(C, dtype=torch.float64, device="cuda").index_add_(0, cell, s * s).cpu().tolist()
             # the same column as the cancelling float64 values through the fast kernel's float64 accumulators
-            got2, names2 = launched(lambda: go([("AggSum_float64", canc)])[0])
+            got2, names2 = _heavy_bin(grid, [("AggSum_float64", canc)])[0], fresh_kernels["13_f64"]
             assert_ran(names2, r"k_binby_fast<float, 1, double, true, true>")
             cancel = got2[inner]
         else:
@@ -296,25 +345,27 @@ def test_heavy_cells_through_both_smem_kernels():
             assert abs(Fraction(float(cancel[c])) - exact) <= Fraction(gamma(k[c])) * mag, (C, c, float(cancel[c]), float(exact))
 
 
-def test_count_cell_past_2p32():
-    """one cell counted past 2^32 by three bin() calls over the same 1.5e9-row device column"""
+COUNT_N = 1_500_000_000
+
+
+def _count_past_2p32():
     import torch
     from vaex_b200 import superagg
-    n = 1_500_000_000
-    x = torch.zeros(n, dtype=torch.uint8, device="cuda")
+    x = torch.zeros(COUNT_N, dtype=torch.uint8, device="cuda")
     b = superagg.BinnerOrdinal_uint8(1, "x", 1, 0, False, False)
     grid = superagg.Grid([b])
     b.set_data(0, x)
+    agg = superagg.AggCount_int64(grid, 1, 1)
+    agg.clear_data_mask(0)
+    for _ in range(3):
+        grid.bin(0, [agg], COUNT_N)
+    return agg.get_result()
 
-    def go():
-        agg = superagg.AggCount_int64(grid, 1, 1)
-        agg.clear_data_mask(0)
-        for _ in range(3):
-            grid.bin(0, [agg], n)
-        return agg.get_result()
-    got, names = launched(go)
-    assert_ran(names, r"k_binby<true, true>")
-    assert got.tolist() == [3 * n, 0, 0]
+
+def test_count_cell_past_2p32(fresh_kernels):
+    """one cell counted past 2^32 by three bin() calls over the same 1.5e9-row device column"""
+    assert_ran(fresh_kernels["count_2p32"], r"k_binby<true, true>")
+    assert _count_past_2p32().tolist() == [3 * COUNT_N, 0, 0]
 
 
 # ---- the edge corpus through whatever kernel it selects, and the golden edge cases ------------------------------------------
@@ -365,3 +416,7 @@ def test_signed_zero_min_max_rule(oracle):
         assert np.signbit(got[0].ravel()[2]) and not np.signbit(got[1].ravel()[2]), v
     binners, aggs, n, expected = golden_util.binby_case(EDGES["kat_minmax_signed_zeros"])
     assert np.signbit(expected[0].ravel()[2]) and np.signbit(expected[1].ravel()[2])  # the reference: the last-arriving -0.0
+
+
+if __name__ == "__main__":  # the profiling half of the heavy-cells and count-past-2^32 tests, in a process of its own
+    _record_fresh_kernels(sys.argv[1])

@@ -323,6 +323,13 @@ def column(ar, expected_itemsize=None):
     return c
 
 
+def memspace(*columns):
+    """The memspace of a call over `columns` (None entries are skipped): HOST or DEVICE when every column lives there, MIXED when
+    host and device columns meet (the library then classifies every pointer), HOST for a call without columns."""
+    spaces = {c.memspace for c in columns if c is not None}
+    return spaces.pop() if len(spaces) == 1 else MEM_MIXED if spaces else MEM_HOST
+
+
 def mask_column(ar):
     """uint8/bool mask -> Column (bool viewed as uint8)."""
     cai = getattr(ar, "__cuda_array_interface__", None)

@@ -141,7 +141,7 @@ void ctx_release(b200_ctx *ctx, void *p, size_t bytes) {
     cudaFree(p);
 }
 
-bool is_device_pointer(const void *p) {
+static bool is_device_pointer(const void *p) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
         cudaGetLastError();
@@ -150,83 +150,123 @@ bool is_device_pointer(const void *p) {
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
-void Stager::plan(const void *p, size_t bytes) {
-    if (!p || memspace == B200_MEM_DEVICE)
+static uint64_t now_ns() {
+    return (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+CallFrame::CallFrame(b200_ctx *c, int slot, int memspace, uint32_t flags, const char *call)
+    : ctx(c), call_(call), memspace_(memspace), async_host_((flags & B200_FLAG_ASYNC_HOST) != 0) {
+    if (!ctx || slot < 0 || slot >= ctx->nslots) {
+        set_error("%s: invalid slot %d (the context has %d)", call, slot, ctx ? ctx->nslots : 0);
+        rc = B200_ERR_INVALID;
         return;
-    if (memspace == B200_MEM_MIXED && is_device_pointer(p))
+    }
+    if (memspace < B200_MEM_HOST || memspace > B200_MEM_MIXED) {
+        set_error("%s: invalid memspace %d", call, memspace);
+        rc = B200_ERR_INVALID;
         return;
-    for (auto &e : entries)
+    }
+    const cudaError_t e = cudaSetDevice(ctx->device);
+    if (e != cudaSuccess) {
+        rc = cuda_fail(e, call, __FILE__, __LINE__);
+        return;
+    }
+    sl = ctx->slots[slot];
+    st = sl->stream;
+    lock_ = std::unique_lock<std::mutex>(sl->mu);
+    if (memspace == B200_MEM_HOST)
+        t0_ = now_ns();
+}
+
+CallFrame::~CallFrame() {
+    if (t0_)
+        sl->host_ns[3] += now_ns() - t0_, sl->host_calls++;
+}
+
+bool CallFrame::on_device(const void *p) const { return memspace_ == B200_MEM_DEVICE || (memspace_ == B200_MEM_MIXED && is_device_pointer(p)); }
+
+bool CallFrame::result_on_device(const void *p) const { return memspace_ == B200_MEM_DEVICE || is_device_pointer(p); }
+
+void CallFrame::plan(const void *p, size_t bytes) {
+    if (!p || on_device(p))
+        return;
+    for (auto &e : entries_)
         if (e.host == p) { // the same column used twice (e.g. binby x and sum x) is copied once
             e.bytes = std::max(e.bytes, bytes);
             return;
         }
-    entries.push_back(Entry{p, bytes, nullptr});
+    entries_.push_back(Entry{p, bytes, nullptr});
 }
 
-int Stager::commit() {
-    if (memspace == B200_MEM_DEVICE || entries.empty())
+int CallFrame::commit() {
+    if (entries_.empty())
         return B200_OK;
-    need = 0;
-    for (auto &e : entries)
+    size_t need = 0;
+    for (auto &e : entries_)
         need += align_up(e.bytes, 256);
-    B200_CHECK(slot_reserve(ctx, slot, need));
+    B200_CHECK(slot_reserve(ctx, sl, need));
     size_t off = 0;
     // MIXED keeps per-column copies (some columns are device pointers and were not planned); HOST chunks whose buffers die with
     // the call go through the slot's page-locked bounce ring
-    const bool bounce = !async_host && memspace == B200_MEM_HOST;
-    if (bounce) {
+    if (!async_host_ && memspace_ == B200_MEM_HOST) {
         // B200_BOUNCE_PIECE_KB / B200_BOUNCE_COUNT: ring geometry (defaults 4 MB x 4)
         static const size_t piece = getenv("B200_BOUNCE_PIECE_KB") ? std::max<size_t>(64, atol(getenv("B200_BOUNCE_PIECE_KB"))) << 10 : 4u << 20;
         static const unsigned count = getenv("B200_BOUNCE_COUNT") ? std::min<unsigned>(Slot::kBounceMax, std::max(2, atoi(getenv("B200_BOUNCE_COUNT")))) : 4u;
-        using clk = std::chrono::steady_clock;
-        auto ns = [](clk::time_point a, clk::time_point b) { return (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(b - a).count(); };
-        for (auto &e : entries) {
-            e.dev = static_cast<char *>(slot->stage) + off;
+        for (auto &e : entries_) {
+            e.dev = static_cast<char *>(sl->stage) + off;
             for (size_t q = 0; q < e.bytes; q += piece) {
                 const size_t len = std::min(piece, e.bytes - q);
-                const unsigned b = slot->bounce_next++ % count;
-                const auto t0 = clk::now();
-                if (slot->bounce_cap[b] < piece) {
-                    if (slot->bounce[b]) {
-                        B200_CUDA(cudaEventSynchronize(slot->bounce_done[b]));
-                        B200_CUDA(cudaFreeHost(slot->bounce[b]));
-                        slot->bounce[b] = nullptr, slot->bounce_cap[b] = 0;
+                const unsigned b = sl->bounce_next++ % count;
+                const uint64_t t0 = now_ns();
+                if (sl->bounce_cap[b] < piece) {
+                    if (sl->bounce[b]) {
+                        B200_CUDA(cudaEventSynchronize(sl->bounce_done[b]));
+                        B200_CUDA(cudaFreeHost(sl->bounce[b]));
+                        sl->bounce[b] = nullptr, sl->bounce_cap[b] = 0;
                     }
-                    B200_CUDA(cudaHostAlloc(&slot->bounce[b], piece, cudaHostAllocPortable));
-                    slot->bounce_cap[b] = piece;
-                    if (!slot->bounce_done[b])
-                        B200_CUDA(cudaEventCreateWithFlags(&slot->bounce_done[b], cudaEventDisableTiming));
+                    B200_CUDA(cudaHostAlloc(&sl->bounce[b], piece, cudaHostAllocPortable));
+                    sl->bounce_cap[b] = piece;
+                    if (!sl->bounce_done[b])
+                        B200_CUDA(cudaEventCreateWithFlags(&sl->bounce_done[b], cudaEventDisableTiming));
                 } else {
-                    B200_CUDA(cudaEventSynchronize(slot->bounce_done[b])); // the copy that last read this piece has finished
+                    B200_CUDA(cudaEventSynchronize(sl->bounce_done[b])); // the copy that last read this piece has finished
                 }
-                const auto t1 = clk::now();
-                copy_to_ring(slot->bounce[b], static_cast<const char *>(e.host) + q, len);
-                const auto t2 = clk::now();
-                B200_CUDA(cudaMemcpyAsync(static_cast<char *>(e.dev) + q, slot->bounce[b], len, cudaMemcpyHostToDevice, slot->stream));
-                B200_CUDA(cudaEventRecord(slot->bounce_done[b], slot->stream));
-                const auto t3 = clk::now();
-                slot->host_ns[0] += ns(t0, t1), slot->host_ns[1] += ns(t1, t2), slot->host_ns[2] += ns(t2, t3), slot->host_pieces++;
+                const uint64_t t1 = now_ns();
+                copy_to_ring(sl->bounce[b], static_cast<const char *>(e.host) + q, len);
+                const uint64_t t2 = now_ns();
+                B200_CUDA(cudaMemcpyAsync(static_cast<char *>(e.dev) + q, sl->bounce[b], len, cudaMemcpyHostToDevice, st));
+                B200_CUDA(cudaEventRecord(sl->bounce_done[b], st));
+                const uint64_t t3 = now_ns();
+                sl->host_ns[0] += t1 - t0, sl->host_ns[1] += t2 - t1, sl->host_ns[2] += t3 - t2, sl->host_pieces++;
             }
             off += align_up(e.bytes, 256);
         }
         return B200_OK;
     }
-    for (auto &e : entries) {
-        e.dev = static_cast<char *>(slot->stage) + off;
+    for (auto &e : entries_) {
+        e.dev = static_cast<char *>(sl->stage) + off;
         off += align_up(e.bytes, 256);
         if (e.bytes)
-            B200_CUDA(cudaMemcpyAsync(e.dev, e.host, e.bytes, cudaMemcpyHostToDevice, slot->stream));
+            B200_CUDA(cudaMemcpyAsync(e.dev, e.host, e.bytes, cudaMemcpyHostToDevice, st));
     }
     return B200_OK;
 }
 
-const void *Stager::dev(const void *p) const {
-    if (!p || memspace == B200_MEM_DEVICE)
+const void *CallFrame::dev(const void *p) const {
+    if (!p || memspace_ == B200_MEM_DEVICE)
         return p;
-    for (auto &e : entries)
+    for (auto &e : entries_)
         if (e.host == p)
             return e.dev;
-    return memspace == B200_MEM_MIXED ? p : nullptr; // MIXED: not planned == already on the device
+    return memspace_ == B200_MEM_MIXED ? p : nullptr; // MIXED: not planned == already on the device
+}
+
+int CallFrame::finish(bool wait) {
+    for (Result &r : results_)
+        B200_CUDA(cudaMemcpyAsync(r.host, r.buf, r.bytes, cudaMemcpyDeviceToHost, st));
+    if (wait || !results_.empty() || (memspace_ == B200_MEM_MIXED && !async_host_))
+        B200_CUDA(cudaStreamSynchronize(st));
+    return B200_OK;
 }
 
 // identity element of an aggregator's device cell
@@ -370,10 +410,6 @@ int b200_ctx_create(int device, int nslots, b200_ctx **out) {
         cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
         if (e == cudaSuccess)
             e = cudaEventCreateWithFlags(&s->h2d_done, cudaEventDisableTiming);
-        if (e == cudaSuccess)
-            e = cudaMallocHost(&s->pinned, 4096);
-        if (e == cudaSuccess)
-            e = cudaMalloc(&s->dscratch, 4096);
         if (e != cudaSuccess) {
             b200_ctx_destroy(ctx);
             return cuda_fail(e, "b200_ctx_create: slot resources", __FILE__, __LINE__);
@@ -392,8 +428,6 @@ int b200_ctx_destroy(b200_ctx *ctx) {
             cudaStreamSynchronize(s->stream);
         cudaFree(s->stage);
         cudaFree(s->scratch);
-        cudaFree(s->dscratch);
-        cudaFreeHost(s->pinned);
         for (int b = 0; b < Slot::kBounceMax; b++) {
             if (s->bounce[b])
                 cudaFreeHost(s->bounce[b]);
@@ -897,15 +931,14 @@ static int bin_nunique(b200_ctx *ctx, Slot *sl, b200_agg *a, const DevBinner *db
 
 int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, const b200_agg_input *aggs, int naggs, int64_t nrows,
              int64_t row_offset, int memspace, uint32_t flags) {
-    if (!ctx || slot < 0 || slot >= ctx->nslots || nbinners < 0 || nbinners > B200_MAX_BINNERS || naggs < 0 || nrows < 0 || (nbinners && !binners) ||
-        (naggs && !aggs)) {
-        set_error("b200_bin: invalid argument (slot %d of %d, %d binners, %d aggregators, %lld rows)", slot, ctx ? ctx->nslots : 0, nbinners, naggs,
-                  (long long)nrows);
+    if (nbinners < 0 || nbinners > B200_MAX_BINNERS || naggs < 0 || nrows < 0 || (nbinners && !binners) || (naggs && !aggs)) {
+        set_error("b200_bin: invalid argument (%d binners, %d aggregators, %lld rows)", nbinners, naggs, (long long)nrows);
         return B200_ERR_INVALID;
     }
+    CallFrame call(ctx, slot, memspace, flags, "b200_bin");
+    B200_CHECK(call.rc);
     if (nrows == 0 || naggs == 0)
         return B200_OK;
-    B200_CUDA(cudaSetDevice(ctx->device));
 
     // grid layout: first binner fastest (src/agg.hpp:63-73)
     DevBinner db[B200_MAX_BINNERS];
@@ -967,53 +1000,41 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
         }
     }
 
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    cudaStream_t st = sl->stream;
-    struct HostTimer { // wall time of HOST calls on this slot, for b200_ctx_host_stats
-        Slot *s;
-        std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-        ~HostTimer() {
-            if (s)
-                s->host_ns[3] += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count(), s->host_calls++;
-        }
-    } host_timer{memspace == B200_MEM_HOST ? sl : nullptr};
+    Slot *sl = call.sl;
+    cudaStream_t st = call.st;
 
     // stage host columns (each distinct pointer once)
-    Stager stg{ctx, sl, memspace};
-    stg.async_host = (flags & B200_FLAG_ASYNC_HOST) != 0;
     for (int i = 0; i < nbinners; i++) {
-        stg.plan(binners[i].data, (size_t)nrows * db[i].isz);
+        call.plan(binners[i].data, (size_t)nrows * db[i].isz);
         if (binners[i].mask)
-            stg.plan(binners[i].mask, (size_t)nrows);
+            call.plan(binners[i].mask, (size_t)nrows);
     }
     std::vector<StrInput> strs; // string list columns: offsets, the call's byte range, validity (sized on first use)
     for (int k = 0; k < naggs; k++) {
         const b200_agg *a = aggs[k].agg;
         if (a->op == B200_AGG_LIST_STRING) {
             strs.resize(naggs);
-            B200_CHECK(plan_strings(sl, stg, static_cast<const int64_t *>(aggs[k].data), static_cast<const uint8_t *>(aggs[k].order), aggs[k].mask, nrows,
-                                    memspace, &strs[k]));
+            B200_CHECK(plan_strings(call, static_cast<const int64_t *>(aggs[k].data), static_cast<const uint8_t *>(aggs[k].order), aggs[k].mask, nrows, &strs[k]));
             continue;
         }
         if (aggs[k].data)
-            stg.plan(aggs[k].data, (size_t)nrows * dtype_size(a->dtype));
+            call.plan(aggs[k].data, (size_t)nrows * dtype_size(a->dtype));
         if (aggs[k].order)
-            stg.plan(aggs[k].order, a->op == B200_AGG_NUNIQUE ? (size_t)nrows : (size_t)nrows * dtype_size(a->dtype2));
+            call.plan(aggs[k].order, a->op == B200_AGG_NUNIQUE ? (size_t)nrows : (size_t)nrows * dtype_size(a->dtype2));
         if (aggs[k].mask) {
             const bool first = a->op == B200_AGG_FIRST || a->op == B200_AGG_LAST;
-            stg.plan(aggs[k].mask, first ? (size_t)std::min<int64_t>(nrows, 1024) : (size_t)nrows);
+            call.plan(aggs[k].mask, first ? (size_t)std::min<int64_t>(nrows, 1024) : (size_t)nrows);
         }
     }
-    B200_CHECK(stg.commit());
+    B200_CHECK(call.commit());
     bool vec = true;
     auto chk = [&](const void *p) {
         if (p && (reinterpret_cast<uintptr_t>(p) & 15))
             vec = false;
     };
     for (int i = 0; i < nbinners; i++) {
-        db[i].data = stg.dev(binners[i].data);
-        db[i].mask = static_cast<const uint8_t *>(stg.dev(binners[i].mask));
+        db[i].data = call.dev(binners[i].data);
+        db[i].mask = static_cast<const uint8_t *>(call.dev(binners[i].mask));
         chk(db[i].data);
         chk(db[i].mask);
     }
@@ -1070,9 +1091,9 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
             fp.isz2 = dtype_size(a->dtype2);
             fp.byteswap = a->byteswap;
             fp.invert = a->op == B200_AGG_LAST;
-            fp.data = stg.dev(aggs[k].data);
-            fp.order = stg.dev(aggs[k].order);
-            fp.mask = static_cast<const uint8_t *>(stg.dev(aggs[k].mask));
+            fp.data = call.dev(aggs[k].data);
+            fp.order = call.dev(aggs[k].order);
+            fp.mask = static_cast<const uint8_t *>(call.dev(aggs[k].mask));
             fp.grid = a->grid;
             fp.order_grid = a->order;
             fp.state = static_cast<unsigned long long *>(a->state.get());
@@ -1089,17 +1110,17 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
             continue;
         }
         if (a->op == B200_AGG_LIST_STRING) {
-            resolve_strings(stg, static_cast<const int64_t *>(aggs[k].data), static_cast<const uint8_t *>(aggs[k].order), aggs[k].mask, &strs[k]);
+            resolve_strings(call, static_cast<const int64_t *>(aggs[k].data), static_cast<const uint8_t *>(aggs[k].order), aggs[k].mask, &strs[k]);
             B200_CHECK(bin_list_string(ctx, sl, a, db, nbinners, strs[k], nrows, vec));
             continue;
         }
         if (a->op == B200_AGG_LIST) {
-            B200_CHECK(bin_list(ctx, sl, a, db, nbinners, stg.dev(aggs[k].data), static_cast<const uint8_t *>(stg.dev(aggs[k].mask)), nrows, vec));
+            B200_CHECK(bin_list(ctx, sl, a, db, nbinners, call.dev(aggs[k].data), static_cast<const uint8_t *>(call.dev(aggs[k].mask)), nrows, vec));
             continue;
         }
         if (a->op == B200_AGG_NUNIQUE) {
-            B200_CHECK(bin_nunique(ctx, sl, a, db, nbinners, stg.dev(aggs[k].data), static_cast<const uint8_t *>(stg.dev(aggs[k].mask)),
-                                   static_cast<const uint8_t *>(stg.dev(aggs[k].order)), nrows, vec));
+            B200_CHECK(bin_nunique(ctx, sl, a, db, nbinners, call.dev(aggs[k].data), static_cast<const uint8_t *>(call.dev(aggs[k].mask)),
+                                   static_cast<const uint8_t *>(call.dev(aggs[k].order)), nrows, vec));
             continue;
         }
         DevAgg &d = p.a[p.na++];
@@ -1111,21 +1132,14 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
         d.cell_dtype = a->cell_dtype;
         d.moment = a->moment;
         d.init_bits = agg_init_bits(a->op, a->cell_dtype);
-        d.data = stg.dev(aggs[k].data);
-        d.mask = static_cast<const uint8_t *>(stg.dev(aggs[k].mask));
+        d.data = call.dev(aggs[k].data);
+        d.mask = static_cast<const uint8_t *>(call.dev(aggs[k].mask));
         d.grid = a->grid;
         if (p.na == B200_MAX_AGGS)
             B200_CHECK(flush());
     }
     B200_CHECK(flush());
-
-    if (memspace == B200_MEM_MIXED && !(flags & B200_FLAG_ASYNC_HOST)) {
-        // MIXED copies straight from the caller's host buffers, which are only valid during the call (vaex/cpu.py:708-710).
-        // Plain HOST chunks were memcpy'd into the slot's page-locked bounce ring: nothing of the caller's is read after return,
-        // so there is no wait here and the next chunk (another slot, or this one) overlaps this chunk's copy and kernels.
-        B200_CUDA(cudaStreamSynchronize(st));
-    }
-    return B200_OK;
+    return call.finish();
 }
 
 } // extern "C"

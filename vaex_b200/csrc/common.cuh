@@ -79,7 +79,6 @@ struct Slot {
     cudaEvent_t h2d_done = nullptr;
     void *stage = nullptr; // device staging arena for host chunks
     size_t stage_cap = 0;
-    void *pinned = nullptr; // small pinned scratch (results of reductions)
     // host-chunk ingestion: a ring of kBounce page-locked pieces of kBouncePiece bytes.  The calling thread memcpy's a host column
     // piece by piece into the ring and every piece travels to the arena with its own asynchronous copy, so the call returns without
     // waiting for the device (the caller's buffer is only valid during the call, vaex/cpu.py:708-710).  The ring is small on
@@ -91,9 +90,8 @@ struct Slot {
     cudaEvent_t bounce_done[kBounceMax] = {};
     unsigned bounce_next = 0;
     // wall-clock nanoseconds of the host-chunk path on this slot (b200_ctx_host_stats): waiting for a ring piece, memcpy into it,
-    // enqueueing its copy, the whole of b200_bin; pieces and calls
+    // enqueueing its copy, the whole of the HOST call; pieces and calls
     uint64_t host_ns[4] = {0, 0, 0, 0}, host_pieces = 0, host_calls = 0;
-    void *dscratch = nullptr;
     void *scratch = nullptr; // partition scratch (ringcount pool + list tables, tilesort buckets)
     size_t scratch_cap = 0;
     // the last ringcount batch on this slot, for b200_ctx_path_stats (device pointers into `scratch`)
@@ -220,28 +218,75 @@ struct b200_agg {
 
 namespace b200 {
 
-// staging: make `n` bytes starting at host/device pointer available on the device for this slot
-struct Stager {
-    b200_ctx *ctx;
-    Slot *slot;
-    int memspace;
-    bool async_host = false; // the caller keeps its host buffers alive until b200_ctx_sync(slot): copy straight from them
-    size_t used = 0;
+// The frame of one per-slot library call: how it reads the caller's memory, where its results land and when it may return.
+// Construction checks the slot (B200_ERR_INVALID naming the call, in `rc`), sets the device and takes the slot's lock for the
+// frame's lifetime.  The slot lock is taken before any set, aggregator or statistic lock, in every call.
+//
+// Inputs, two-phase: plan() every column, then commit() stages the host ones into the slot's arena in one allocation and dev()
+// gives each column's device pointer.  HOST columns go through the slot's page-locked bounce ring (Slot::bounce); MIXED columns
+// are classified one by one and the host ones are copied straight from the caller's buffers; DEVICE columns are used in place.
+// Results: out() gives the device pointer a result is written to, the caller's own or a temporary copied back by finish().
+//
+// The return rule, applied by finish(): the call waits for the slot's stream when a result goes to host memory, when MIXED
+// inputs were copied straight from the caller's host buffers and B200_FLAG_ASYNC_HOST does not keep them alive (they are valid
+// only during the call, vaex/cpu.py:708-710), or when the call asks to wait.  HOST inputs were memcpy'd into the bounce ring and
+// DEVICE inputs stay the caller's: nothing of the caller's is read after return, so the next chunk (this slot or another)
+// overlaps this one's copies and kernels.
+class CallFrame {
+  public:
+    CallFrame(b200_ctx *ctx, int slot, int memspace, uint32_t flags, const char *call);
+    ~CallFrame();
+    CallFrame(const CallFrame &) = delete;
+    CallFrame &operator=(const CallFrame &) = delete;
+
+    int rc = B200_OK; // check before anything else: nothing is locked unless it is B200_OK
+    b200_ctx *const ctx;
+    Slot *sl = nullptr;
+    cudaStream_t st = nullptr;
+
+    // whether an input column lives on the device: every column of a DEVICE call, none of a HOST call, each on its own in MIXED
+    bool on_device(const void *p) const;
+    // whether a result pointer lives on the device: every one of a DEVICE call, each on its own otherwise
+    bool result_on_device(const void *p) const;
+    void plan(const void *p, size_t bytes);
+    int commit();
+    const void *dev(const void *p) const;
+    // the device pointer `bytes` of a result are written to: `p` itself when on_device, otherwise a temporary on the slot's
+    // stream that finish() copies to `p`
+    template <typename T> int out(void *p, size_t bytes, bool on_device, T **dev) {
+        if (on_device) {
+            *dev = static_cast<T *>(p);
+            return B200_OK;
+        }
+        DevBuf<> buf;
+        B200_CHECK(buf.alloc(ctx, bytes, call_, st));
+        *dev = static_cast<T *>(buf.get());
+        results_.push_back(Result{p, bytes, std::move(buf)});
+        return B200_OK;
+    }
+    int finish(bool wait = false);
+
+  private:
     struct Entry {
         const void *host;
         size_t bytes;
         void *dev;
     };
-    std::vector<Entry> entries;
-    size_t need = 0;
-    // two-phase: plan() every column, then commit() allocates once and issues the copies
-    void plan(const void *p, size_t bytes);
-    int commit();
-    const void *dev(const void *p) const;
+    struct Result {
+        void *host;
+        size_t bytes;
+        DevBuf<> buf;
+    };
+    const char *call_;
+    int memspace_;
+    bool async_host_;
+    std::unique_lock<std::mutex> lock_;
+    uint64_t t0_ = 0;
+    std::vector<Entry> entries_;
+    std::vector<Result> results_;
 };
 
 int slot_reserve(b200_ctx *ctx, Slot *s, size_t bytes);
-bool is_device_pointer(const void *p);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 

@@ -367,14 +367,15 @@ using namespace b200;
 
 extern "C" int b200_eval(b200_ctx *ctx, int slot, const b200_expr_op *prog, int nops, const b200_expr_input *inputs, int ninputs, b200_set *const *sets,
                          int nsets, int64_t nrows, int memspace, int out_dtype, void *out_device) {
-    if (!ctx || slot < 0 || slot >= ctx->nslots || !prog || nops < 1 || nops > kMaxOps || ninputs < 0 || ninputs > kMaxInputs || nsets < 0 ||
-        nsets > kMaxSets || nrows < 0 || out_dtype < 0 || out_dtype >= B200_NDTYPE || (nrows && !out_device)) {
+    if (!prog || nops < 1 || nops > kMaxOps || ninputs < 0 || ninputs > kMaxInputs || nsets < 0 || nsets > kMaxSets || nrows < 0 || out_dtype < 0 ||
+        out_dtype >= B200_NDTYPE || (nrows && !out_device)) {
         set_error("b200_eval: invalid argument (%d ops, %d inputs, %d sets)", nops, ninputs, nsets);
         return B200_ERR_INVALID;
     }
+    CallFrame call(ctx, slot, memspace, 0, "b200_eval");
+    B200_CHECK(call.rc);
     if (!nrows)
         return B200_OK;
-    B200_CUDA(cudaSetDevice(ctx->device));
     EvalParams p;
     memset(&p, 0, sizeof p);
     // validate the program: stack discipline, operand indices (a malformed program must not read out of bounds on the device)
@@ -428,22 +429,19 @@ extern "C" int b200_eval(b200_ctx *ctx, int slot, const b200_expr_op *prog, int 
         set_error("b200_eval: the program leaves %d values (stack depth %d, limit %d)", depth, maxdepth, kStack);
         return B200_ERR_INVALID;
     }
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    Stager stg{ctx, sl, memspace};
     for (int k = 0; k < ninputs; k++) {
         if (inputs[k].dtype < 0 || inputs[k].dtype >= B200_NDTYPE || !inputs[k].data) {
             set_error("b200_eval: input %d: %s", k, inputs[k].data ? "unknown dtype" : "data not set");
             return B200_ERR_INVALID;
         }
-        stg.plan(inputs[k].data, (size_t)nrows * dtype_size(inputs[k].dtype));
+        call.plan(inputs[k].data, (size_t)nrows * dtype_size(inputs[k].dtype));
     }
-    B200_CHECK(stg.commit());
+    B200_CHECK(call.commit());
     p.nops = nops;
     p.ninputs = ninputs;
     memcpy(p.ops, prog, sizeof(b200_expr_op) * nops);
     for (int k = 0; k < ninputs; k++) {
-        p.in[k] = stg.dev(inputs[k].data);
+        p.in[k] = call.dev(inputs[k].data);
         p.in_dtype[k] = inputs[k].dtype;
     }
     for (int k = 0; k < nsets; k++) {
@@ -461,30 +459,25 @@ extern "C" int b200_eval(b200_ctx *ctx, int slot, const b200_expr_op *prog, int 
     p.out = out_device;
     const long long want = (nrows + 255) / 256;
     const int blocks = (int)std::min<long long>(want, (long long)ctx->sm_count * 16);
-    k_eval<<<blocks, 256, 0, sl->stream>>>(p);
+    k_eval<<<blocks, 256, 0, call.st>>>(p);
     B200_CUDA(cudaGetLastError());
-    if (memspace == B200_MEM_MIXED)
-        B200_CUDA(cudaStreamSynchronize(sl->stream)); // MIXED copies straight from the caller's host buffers
-    return B200_OK;
+    return call.finish();
 }
 
 extern "C" int b200_compact(b200_ctx *ctx, int slot, const uint8_t *keep, int ncols, const void *const *cols, const int32_t *dtypes, int64_t nrows,
                             int memspace, void *const *outs_device, int64_t *count_out) {
-    if (!ctx || slot < 0 || slot >= ctx->nslots || ncols < 0 || ncols > kMaxCompactCols || nrows < 0 || !count_out || (nrows && !keep) ||
-        (ncols && (!cols || !dtypes || !outs_device))) {
+    if (ncols < 0 || ncols > kMaxCompactCols || nrows < 0 || !count_out || (nrows && !keep) || (ncols && (!cols || !dtypes || !outs_device))) {
         set_error("b200_compact: invalid argument");
         return B200_ERR_INVALID;
     }
+    CallFrame call(ctx, slot, memspace, 0, "b200_compact");
+    B200_CHECK(call.rc);
     *count_out = 0;
     if (!nrows)
         return B200_OK;
-    B200_CUDA(cudaSetDevice(ctx->device));
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    Stager stg{ctx, sl, memspace};
+    cudaStream_t st = call.st;
     const unsigned nblk = (unsigned)((nrows + kCompactBlock - 1) / kCompactBlock);
-    // the block counters ride at the end of the staging arena request (device scratch only: never copied from the host)
-    stg.plan(keep, (size_t)nrows);
+    call.plan(keep, (size_t)nrows);
     CompactParams p;
     memset(&p, 0, sizeof p);
     p.ncols = ncols;
@@ -494,25 +487,22 @@ extern "C" int b200_compact(b200_ctx *ctx, int slot, const uint8_t *keep, int nc
             return B200_ERR_INVALID;
         }
         p.isz[c] = dtype_size(dtypes[c]);
-        stg.plan(cols[c], (size_t)nrows * p.isz[c]);
+        call.plan(cols[c], (size_t)nrows * p.isz[c]);
     }
-    B200_CHECK(stg.commit());
+    B200_CHECK(call.commit());
     for (int c = 0; c < ncols; c++) {
-        p.in[c] = stg.dev(cols[c]);
+        p.in[c] = call.dev(cols[c]);
         p.out[c] = outs_device[c];
     }
-    const uint8_t *d_keep = static_cast<const uint8_t *>(stg.dev(keep));
+    const uint8_t *d_keep = static_cast<const uint8_t *>(call.dev(keep));
     DevBuf<unsigned> d_counts;
-    B200_CHECK(d_counts.alloc(ctx, (size_t)nblk * 4 + 16, "b200_compact", sl->stream));
-    unsigned long long *d_total = reinterpret_cast<unsigned long long *>(sl->dscratch);
-    k_keep_count<<<nblk, kCompactBlock, 0, sl->stream>>>(d_keep, nrows, d_counts);
-    k_scan_u32<<<1, 1024, 0, sl->stream>>>(d_counts, nblk, d_total);
+    B200_CHECK(d_counts.alloc(ctx, (size_t)nblk * 4 + 16, "b200_compact", st));
+    unsigned long long *d_total;
+    B200_CHECK(call.out(count_out, 8, false, &d_total));
+    k_keep_count<<<nblk, kCompactBlock, 0, st>>>(d_keep, nrows, d_counts);
+    k_scan_u32<<<1, 1024, 0, st>>>(d_counts, nblk, d_total);
     if (ncols)
-        k_compact<<<nblk, kCompactBlock, 0, sl->stream>>>(d_keep, nrows, d_counts, p);
+        k_compact<<<nblk, kCompactBlock, 0, st>>>(d_keep, nrows, d_counts, p);
     B200_CUDA(cudaGetLastError());
-    unsigned long long total = 0;
-    B200_CUDA(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, sl->stream));
-    B200_CUDA(cudaStreamSynchronize(sl->stream));
-    *count_out = (int64_t)total;
-    return B200_OK;
+    return call.finish();
 }

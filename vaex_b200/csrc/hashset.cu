@@ -734,7 +734,7 @@ int b200_set_destroy(b200_set *s) {
 
 int b200_set_update(b200_set *s, int slot, const void *keys, const uint8_t *masks, int64_t nrows, int64_t start_index, int return_values,
                     int64_t *out_values, int16_t *out_map_index, int memspace, uint32_t flags) {
-    if (!s || slot < 0 || slot >= s->ctx->nslots || nrows < 0 || (nrows && !keys)) {
+    if (!s || nrows < 0 || (nrows && !keys)) {
         set_error("b200_set_update: invalid argument");
         return B200_ERR_INVALID;
     }
@@ -746,35 +746,30 @@ int b200_set_update(b200_set *s, int slot, const void *keys, const uint8_t *mask
         set_error("b200_set_update: more than 2^40 rows in one call");
         return B200_ERR_UNSUPPORTED;
     }
-    B200_CUDA(cudaSetDevice(s->ctx->device));
-    Slot *sl = s->ctx->slots[slot];
+    CallFrame call(s->ctx, slot, memspace, flags, "b200_set_update");
+    B200_CHECK(call.rc);
     std::lock_guard<std::mutex> g(s->mu);
-    std::lock_guard<std::mutex> gs(sl->mu);
-    Stager stg{s->ctx, sl, memspace};
+    cudaStream_t st = call.st;
     const size_t isz = dtype_size(s->dtype);
-    stg.plan(keys, (size_t)nrows * isz);
+    call.plan(keys, (size_t)nrows * isz);
     if (masks)
-        stg.plan(masks, (size_t)nrows);
-    B200_CHECK(stg.commit());
-    const void *d_keys = stg.dev(keys);
-    const uint8_t *d_masks = masks ? static_cast<const uint8_t *>(stg.dev(masks)) : nullptr;
+        call.plan(masks, (size_t)nrows);
+    B200_CHECK(call.commit());
+    const void *d_keys = call.dev(keys);
+    const uint8_t *d_masks = masks ? static_cast<const uint8_t *>(call.dev(masks)) : nullptr;
     const bool use_offsets = return_values || start_index != -1;
-    B200_CHECK(set_insert_device(s, sl->stream, d_keys, d_masks, nrows, use_offsets, false, -1));
+    B200_CHECK(set_insert_device(s, st, d_keys, d_masks, nrows, use_offsets, false, -1));
     if (return_values && nrows) {
         B200_CHECK(set_finalize(s));
-        DevBuf<long long> d_vals;
-        DevBuf<short> d_map;
-        B200_CHECK(d_vals.alloc(s->ctx, sizeof(long long) * nrows, "b200_set_update", sl->stream));
-        B200_CHECK(d_map.alloc(s->ctx, sizeof(short) * nrows, "b200_set_update", sl->stream));
-        k_set_values<<<nblocks((unsigned long long)nrows), 256, 0, sl->stream>>>(s->probe, s->probe_cap - 1, s->sentinel_ordinal, s->nan_value, s->null_value,
-                                                                               s->dtype, (int)isz, s->nmaps, s->d_offsets, d_keys, d_masks, nrows, d_vals, d_map);
+        long long *d_vals;
+        short *d_map;
+        B200_CHECK(call.out(out_values, sizeof(long long) * nrows, false, &d_vals));
+        B200_CHECK(call.out(out_map_index, sizeof(short) * nrows, false, &d_map));
+        k_set_values<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->probe, s->probe_cap - 1, s->sentinel_ordinal, s->nan_value, s->null_value, s->dtype,
+                                                                       (int)isz, s->nmaps, s->d_offsets, d_keys, d_masks, nrows, d_vals, d_map);
         B200_CUDA(cudaGetLastError());
-        B200_CUDA(cudaMemcpyAsync(out_values, d_vals, sizeof(long long) * nrows, cudaMemcpyDeviceToHost, sl->stream));
-        B200_CUDA(cudaMemcpyAsync(out_map_index, d_map, sizeof(short) * nrows, cudaMemcpyDeviceToHost, sl->stream));
-        B200_CUDA(cudaStreamSynchronize(sl->stream));
     }
-    (void)flags;
-    return B200_OK;
+    return call.finish();
 }
 
 int b200_set_from_keys(b200_ctx *ctx, int dtype, const void *keys, int64_t nkeys, int64_t null_index, int64_t nan_count, int64_t null_count,
@@ -783,14 +778,12 @@ int b200_set_from_keys(b200_ctx *ctx, int dtype, const void *keys, int64_t nkeys
     B200_CHECK(b200_set_create(ctx, dtype, 1, -1, &s));
     int rc = B200_OK;
     {
-        Slot *sl = ctx->slots[0];
+        CallFrame call(ctx, 0, B200_MEM_HOST, 0, "b200_set_from_keys");
         std::lock_guard<std::mutex> g(s->mu);
-        std::lock_guard<std::mutex> gs(sl->mu);
-        Stager stg{ctx, sl, B200_MEM_HOST};
-        stg.plan(keys, (size_t)nkeys * dtype_size(dtype));
-        rc = stg.commit();
+        call.plan(keys, (size_t)nkeys * dtype_size(dtype));
+        rc = call.rc ? call.rc : call.commit();
         if (!rc && nkeys)
-            rc = set_insert_device(s, sl->stream, stg.dev(keys), nullptr, nkeys, true, true, null_index);
+            rc = set_insert_device(s, call.st, call.dev(keys), nullptr, nkeys, true, true, null_index);
         if (!rc)
             rc = set_finalize(s);
         if (!rc) {
@@ -816,6 +809,8 @@ int b200_set_from_keys(b200_ctx *ctx, int dtype, const void *keys, int64_t nkeys
                 s->null_count = null_count;
             }
         }
+        if (!rc)
+            rc = call.finish();
     }
     if (rc) {
         b200_set_destroy(s);
@@ -862,26 +857,25 @@ int b200_set_merge(b200_set *s, b200_set *const *others, int nothers) {
             o_nan = o->nan_count;
             o_null = o->null_count;
         }
-        Slot *sl = s->ctx->slots[0];
+        CallFrame call(s->ctx, 0, B200_MEM_HOST, 0, "b200_set_merge");
+        B200_CHECK(call.rc);
         std::lock_guard<std::mutex> g(s->mu);
-        std::lock_guard<std::mutex> gs(sl->mu);
         // feed canonical patterns as a 64-bit column of a same-hash dtype: U64 for hashed types keeps hash64(canon)
         // identical; identity-hashed small ints also stay identical because key_hash(dtype, canon) == canon there.
         int saved = s->dtype;
-        Stager stg{s->ctx, sl, B200_MEM_HOST};
-        stg.plan(keys.data(), keys.size() * 8);
+        call.plan(keys.data(), keys.size() * 8);
         if (!weights.empty())
-            stg.plan(weights.data(), weights.size() * 8);
-        B200_CHECK(stg.commit());
+            call.plan(weights.data(), weights.size() * 8);
+        B200_CHECK(call.commit());
         // canonical patterns re-enter through a raw 64-bit view; key_canon(U64) is the identity and the shard hash is
         // evaluated from s->dtype at finalize, so only the column width differs.
         s->dtype = B200_U64;
         s->hold_count_pass = true;
-        int rc = keys.empty() ? B200_OK : set_insert_device(s, sl->stream, stg.dev(keys.data()), nullptr, (int64_t)keys.size(), false, false, -1);
+        int rc = keys.empty() ? B200_OK : set_insert_device(s, call.st, call.dev(keys.data()), nullptr, (int64_t)keys.size(), false, false, -1);
         s->hold_count_pass = false;
         if (!rc && s->counting && !weights.empty()) {
-            k_set_count<<<nblocks(keys.size()), 256, 0, sl->stream>>>(s->table, s->cap - 1, s->counts, s->d_ctr, B200_U64, 8, stg.dev(keys.data()), nullptr,
-                                                                      static_cast<const unsigned long long *>(stg.dev(weights.data())), (long long)keys.size());
+            k_set_count<<<nblocks(keys.size()), 256, 0, call.st>>>(s->table, s->cap - 1, s->counts, s->d_ctr, B200_U64, 8, call.dev(keys.data()), nullptr,
+                                                                   static_cast<const unsigned long long *>(call.dev(weights.data())), (long long)keys.size());
             if (cudaGetLastError() != cudaSuccess)
                 rc = B200_ERR_CUDA;
         }
@@ -889,7 +883,7 @@ int b200_set_merge(b200_set *s, b200_set *const *others, int nothers) {
         B200_CHECK(rc);
         // nan/null: counts add up; a special first seen through a merge takes the next shard-0 ordinal
         unsigned long long h[CTR_N];
-        B200_CHECK(read_ctr(s, sl->stream, h));
+        B200_CHECK(read_ctr(s, call.st, h));
         const unsigned long long tag_base = (unsigned long long)(s->seq - (keys.empty() ? 0 : 1)) << 40;
         if (keys.empty())
             s->seq++;
@@ -903,8 +897,8 @@ int b200_set_merge(b200_set *s, b200_set *const *others, int nothers) {
             if (h[CTR_NULL_TAG] == ~0ull)
                 h[CTR_NULL_TAG] = tag_base | kTagLowMask;
         }
-        B200_CUDA(cudaMemcpyAsync(s->d_ctr, h, sizeof h, cudaMemcpyHostToDevice, sl->stream));
-        B200_CUDA(cudaStreamSynchronize(sl->stream));
+        B200_CUDA(cudaMemcpyAsync(s->d_ctr, h, sizeof h, cudaMemcpyHostToDevice, call.st));
+        B200_CHECK(call.finish(true));
         s->dirty = true;
     }
     return B200_OK;
@@ -976,63 +970,52 @@ int b200_set_ordinal_dtype(b200_set *s) {
     return B200_I64;
 }
 
-static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows, void *out, int out_isz, int memspace) {
-    if (!s || slot < 0 || slot >= s->ctx->nslots || nrows < 0) {
-        set_error("b200_set_map: invalid argument");
+// out: nrows results of out_isz bytes (0: isin's one byte) in host or device memory (CallFrame::result_on_device)
+static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows, void *out, int out_isz, int memspace, uint32_t flags, const char *name) {
+    if (!s || nrows < 0) {
+        set_error("%s: invalid argument", name);
         return B200_ERR_INVALID;
     }
+    CallFrame call(s->ctx, slot, memspace, flags, name);
+    B200_CHECK(call.rc);
     if (!nrows)
         return B200_OK;
-    B200_CUDA(cudaSetDevice(s->ctx->device));
-    Slot *sl = s->ctx->slots[slot];
     std::lock_guard<std::mutex> g(s->mu);
     B200_CHECK(set_finalize(s));
-    std::lock_guard<std::mutex> gs(sl->mu);
-    Stager stg{s->ctx, sl, memspace};
     const size_t isz = dtype_size(s->dtype);
     const size_t osz = out_isz ? out_isz : 1;
-    stg.plan(keys, (size_t)nrows * isz);
-    B200_CHECK(stg.commit());
-    void *d_out = out;
-    DevBuf<> host_out;
-    const bool out_host = memspace == B200_MEM_HOST || (memspace == B200_MEM_MIXED && !is_device_pointer(out));
-    if (out_host) {
-        B200_CHECK(host_out.alloc(s->ctx, nrows * osz, "b200_set_map", sl->stream));
-        d_out = host_out;
-    }
-    k_set_map<<<nblocks((unsigned long long)nrows), 256, 0, sl->stream>>>(s->probe, s->probe_cap - 1, s->sentinel_ordinal,
-                                                                        s->nan_count > 0 ? s->nan_value : -1, s->dtype, (int)isz, stg.dev(keys), nrows, d_out,
-                                                                        out_isz);
+    call.plan(keys, (size_t)nrows * isz);
+    B200_CHECK(call.commit());
+    void *d_out;
+    B200_CHECK(call.out(out, nrows * osz, call.result_on_device(out), &d_out));
+    k_set_map<<<nblocks((unsigned long long)nrows), 256, 0, call.st>>>(s->probe, s->probe_cap - 1, s->sentinel_ordinal, s->nan_count > 0 ? s->nan_value : -1,
+                                                                     s->dtype, (int)isz, call.dev(keys), nrows, d_out, out_isz);
     B200_CUDA(cudaGetLastError());
-    if (out_host) {
-        B200_CUDA(cudaMemcpyAsync(out, d_out, nrows * osz, cudaMemcpyDeviceToHost, sl->stream));
-        B200_CUDA(cudaStreamSynchronize(sl->stream));
-    }
-    return B200_OK;
+    return call.finish();
 }
 
 int b200_set_map_ordinal(b200_set *s, int slot, const void *keys, int64_t nrows, void *out, int memspace, uint32_t flags) {
-    (void)flags;
     int od = b200_set_ordinal_dtype(s);
-    return set_map_common(s, slot, keys, nrows, out, dtype_size(od), memspace);
+    return set_map_common(s, slot, keys, nrows, out, dtype_size(od), memspace, flags, "b200_set_map_ordinal");
 }
 
 // ordered_set::isin (src/hash_primitives.hpp:539-565); NaN is "in" iff the set saw a NaN
 int b200_set_isin(b200_set *s, int slot, const void *keys, int64_t nrows, uint8_t *out, int memspace, uint32_t flags) {
-    (void)flags;
-    return set_map_common(s, slot, keys, nrows, out, 0, memspace);
+    return set_map_common(s, slot, keys, nrows, out, 0, memspace, flags, "b200_set_isin");
 }
 
 int b200_set_combine(b200_ctx *ctx, int slot, int nkeys, b200_set *const *sets, const void *const *keys, const uint8_t *const *masks,
                      const int64_t *multipliers, int64_t nrows, int64_t *out, int memspace, uint32_t flags) {
-    (void)flags;
-    if (!ctx || slot < 0 || slot >= ctx->nslots || nkeys < 1 || nkeys > B200_MAX_COMBINE || !sets || !keys || !multipliers || nrows < 0 || (nrows && !out)) {
+    if (nkeys < 1 || nkeys > B200_MAX_COMBINE || !sets || !keys || !multipliers || nrows < 0 || (nrows && !out)) {
         set_error("b200_set_combine: invalid argument");
         return B200_ERR_INVALID;
     }
+    // flags are not read: a MIXED call waits for its stream whatever they say
+    (void)flags;
+    CallFrame call(ctx, slot, memspace, 0, "b200_set_combine");
+    B200_CHECK(call.rc);
     if (!nrows)
         return B200_OK;
-    B200_CUDA(cudaSetDevice(ctx->device));
     CombineParams p;
     memset(&p, 0, sizeof p);
     p.nkeys = nkeys;
@@ -1053,35 +1036,21 @@ int b200_set_combine(b200_ctx *ctx, int slot, int nkeys, b200_set *const *sets, 
         p.dtype[k] = s->dtype;
         p.isz[k] = (int)dtype_size(s->dtype);
     }
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> gs(sl->mu);
-    Stager stg{ctx, sl, memspace};
     for (int k = 0; k < nkeys; k++) {
-        stg.plan(keys[k], (size_t)nrows * p.isz[k]);
+        call.plan(keys[k], (size_t)nrows * p.isz[k]);
         if (masks && masks[k])
-            stg.plan(masks[k], (size_t)nrows);
+            call.plan(masks[k], (size_t)nrows);
     }
-    B200_CHECK(stg.commit());
+    B200_CHECK(call.commit());
     for (int k = 0; k < nkeys; k++) {
-        p.keys[k] = stg.dev(keys[k]);
-        p.masks[k] = masks && masks[k] ? static_cast<const uint8_t *>(stg.dev(masks[k])) : nullptr;
+        p.keys[k] = call.dev(keys[k]);
+        p.masks[k] = masks && masks[k] ? static_cast<const uint8_t *>(call.dev(masks[k])) : nullptr;
     }
-    long long *d_out = reinterpret_cast<long long *>(out);
-    DevBuf<long long> host_out;
-    const bool out_host = memspace == B200_MEM_HOST || (memspace == B200_MEM_MIXED && !is_device_pointer(out));
-    if (out_host) {
-        B200_CHECK(host_out.alloc(ctx, nrows * 8, "b200_set_combine", sl->stream));
-        d_out = host_out;
-    }
-    k_set_combine<<<nblocks((unsigned long long)nrows), 256, 0, sl->stream>>>(p, nrows, d_out);
+    long long *d_out;
+    B200_CHECK(call.out(out, nrows * 8, call.result_on_device(out), &d_out));
+    k_set_combine<<<nblocks((unsigned long long)nrows), 256, 0, call.st>>>(p, nrows, d_out);
     B200_CUDA(cudaGetLastError());
-    if (out_host) {
-        B200_CUDA(cudaMemcpyAsync(out, d_out, nrows * 8, cudaMemcpyDeviceToHost, sl->stream));
-        B200_CUDA(cudaStreamSynchronize(sl->stream));
-    } else if (memspace != B200_MEM_DEVICE) {
-        B200_CUDA(cudaStreamSynchronize(sl->stream)); // the caller's host key buffers are only valid during the call
-    }
-    return B200_OK;
+    return call.finish();
 }
 
 // hash_base::bytes_used (src/hash_primitives.hpp:62-69): sum over maps of size * (sizeof(key) + sizeof(value))
@@ -1337,7 +1306,7 @@ int b200_strset_create(b200_ctx *ctx, int nmaps, int64_t limit, b200_set **out) 
 
 int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, int return_values,
                        int64_t *out_values, int16_t *out_map_index, int memspace) {
-    if (!s || !s->strings || slot < 0 || slot >= s->ctx->nslots || nrows < 0 || (nrows && !offsets)) {
+    if (!s || !s->strings || nrows < 0 || (nrows && !offsets)) {
         set_error("b200_strset_update: invalid argument");
         return B200_ERR_INVALID;
     }
@@ -1345,14 +1314,12 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
         set_error("b200_strset_update: more than 2^40 rows in one call");
         return B200_ERR_UNSUPPORTED;
     }
-    B200_CUDA(cudaSetDevice(s->ctx->device));
-    Slot *sl = s->ctx->slots[slot];
+    CallFrame call(s->ctx, slot, memspace, 0, "b200_strset_update");
+    B200_CHECK(call.rc);
     std::lock_guard<std::mutex> g(s->mu);
-    std::lock_guard<std::mutex> gs(sl->mu);
-    cudaStream_t st = sl->stream;
-    Stager stg{s->ctx, sl, memspace};
+    cudaStream_t st = call.st;
     StrInput in;
-    B200_CHECK(stage_strings(sl, stg, offsets, bytes, masks, nrows, memspace, &in));
+    B200_CHECK(stage_strings(call, offsets, bytes, masks, nrows, &in));
     // room for the worst case of this call: every row a new key
     {
         uint64_t want = s->cap;
@@ -1407,54 +1374,41 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
     B200_CHECK(str_check_error(s, st));
     if (return_values && nrows) {
         B200_CHECK(str_finalize(s));
-        DevBuf<long long> d_vals;
-        DevBuf<short> d_map;
-        B200_CHECK(d_vals.alloc(s->ctx, sizeof(long long) * nrows, "b200_strset_update", st));
-        B200_CHECK(d_map.alloc(s->ctx, sizeof(short) * nrows, "b200_strset_update", st));
+        long long *d_vals;
+        short *d_map;
+        B200_CHECK(call.out(out_values, sizeof(long long) * nrows, false, &d_vals));
+        B200_CHECK(call.out(out_map_index, sizeof(short) * nrows, false, &d_map));
         k_str_map<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->probe, s->probe_cap - 1, s->d_str_off, s->d_str_len, s->pool,
                                                                     s->null_count > 0 ? s->null_value : -1, s->nmaps, s->d_offsets, in.offsets, in.bytes, in.masks,
                                                                     in.base, nrows, d_vals, d_map, 1);
         B200_CUDA(cudaGetLastError());
-        B200_CUDA(cudaMemcpyAsync(out_values, d_vals, sizeof(long long) * nrows, cudaMemcpyDeviceToHost, st));
-        B200_CUDA(cudaMemcpyAsync(out_map_index, d_map, sizeof(short) * nrows, cudaMemcpyDeviceToHost, st));
-        B200_CUDA(cudaStreamSynchronize(st));
     }
-    B200_CUDA(cudaStreamSynchronize(st)); // the caller's buffers are only valid during the call
-    return B200_OK;
+    return call.finish(true);
 }
 
 /* out: nrows int64 ordinals (-1: not a member; nulls map to the null ordinal), written to host memory or, with out_is_device, to a
  * device buffer on the slot's stream */
 int b200_strset_map_ordinal(b200_set *s, int slot, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, int64_t *out,
                             int memspace, int out_is_device) {
-    if (!s || !s->strings || slot < 0 || slot >= s->ctx->nslots || nrows < 0 || (nrows && (!offsets || !out))) {
+    if (!s || !s->strings || nrows < 0 || (nrows && (!offsets || !out))) {
         set_error("b200_strset_map_ordinal: invalid argument");
         return B200_ERR_INVALID;
     }
+    CallFrame call(s->ctx, slot, memspace, 0, "b200_strset_map_ordinal");
+    B200_CHECK(call.rc);
     if (!nrows)
         return B200_OK;
-    B200_CUDA(cudaSetDevice(s->ctx->device));
-    Slot *sl = s->ctx->slots[slot];
     std::lock_guard<std::mutex> g(s->mu);
-    std::lock_guard<std::mutex> gs(sl->mu);
-    cudaStream_t st = sl->stream;
     B200_CHECK(str_finalize(s));
-    Stager stg{s->ctx, sl, memspace};
     StrInput in;
-    B200_CHECK(stage_strings(sl, stg, offsets, bytes, masks, nrows, memspace, &in));
-    long long *d_out = reinterpret_cast<long long *>(out);
-    DevBuf<long long> host_out;
-    if (!out_is_device) {
-        B200_CHECK(host_out.alloc(s->ctx, sizeof(long long) * nrows, "b200_strset_map_ordinal", st));
-        d_out = host_out;
-    }
-    k_str_map<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->probe, s->probe_cap - 1, s->d_str_off, s->d_str_len, s->pool, s->null_count > 0 ? s->null_value : -1,
-                                                                s->nmaps, s->d_offsets, in.offsets, in.bytes, in.masks, in.base, nrows, d_out, nullptr, 0);
+    B200_CHECK(stage_strings(call, offsets, bytes, masks, nrows, &in));
+    long long *d_out;
+    B200_CHECK(call.out(out, sizeof(long long) * nrows, out_is_device != 0, &d_out));
+    k_str_map<<<nblocks((unsigned long long)nrows), 256, 0, call.st>>>(s->probe, s->probe_cap - 1, s->d_str_off, s->d_str_len, s->pool,
+                                                                     s->null_count > 0 ? s->null_value : -1, s->nmaps, s->d_offsets, in.offsets, in.bytes,
+                                                                     in.masks, in.base, nrows, d_out, nullptr, 0);
     B200_CUDA(cudaGetLastError());
-    if (!out_is_device)
-        B200_CUDA(cudaMemcpyAsync(out, d_out, sizeof(long long) * nrows, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    return B200_OK;
+    return call.finish(true);
 }
 
 /* key_array(): first the byte count, then offsets (int64[count + 1]) + bytes in ordinal order; the null slot is an empty string */

@@ -114,42 +114,40 @@ using namespace b200;
 
 extern "C" int b200_minmax(b200_ctx *ctx, int slot, int dtype, int byteswap, const void *data, const uint8_t *mask, int64_t nrows, int memspace,
                            double *out) {
-    if (!ctx || slot < 0 || slot >= ctx->nslots || dtype < 0 || dtype >= B200_NDTYPE || !out || (nrows && !data)) {
+    if (dtype < 0 || dtype >= B200_NDTYPE || !out || (nrows && !data)) {
         set_error("b200_minmax: invalid argument");
         return B200_ERR_INVALID;
     }
-    B200_CUDA(cudaSetDevice(ctx->device));
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    Stager stg{ctx, sl, memspace};
+    CallFrame call(ctx, slot, memspace, 0, "b200_minmax");
+    B200_CHECK(call.rc);
     const int isz = dtype_size(dtype);
-    stg.plan(data, (size_t)nrows * isz);
+    call.plan(data, (size_t)nrows * isz);
     if (mask)
-        stg.plan(mask, (size_t)nrows);
-    B200_CHECK(stg.commit());
+        call.plan(mask, (size_t)nrows);
+    B200_CHECK(call.commit());
     double init[2] = {INFINITY, -INFINITY}; // StatOpMinMax.init (vaex/tasks.py)
-    double *d = static_cast<double *>(sl->dscratch);
-    B200_CUDA(cudaMemcpyAsync(d, init, sizeof init, cudaMemcpyHostToDevice, sl->stream));
+    double *d;
+    B200_CHECK(call.out(out, sizeof init, false, &d));
+    cudaStream_t st = call.st;
+    B200_CUDA(cudaMemcpyAsync(d, init, sizeof init, cudaMemcpyHostToDevice, st));
     if (nrows) {
-        const void *dd = stg.dev(data);
-        const uint8_t *dm = static_cast<const uint8_t *>(stg.dev(mask));
+        const void *dd = call.dev(data);
+        const uint8_t *dm = static_cast<const uint8_t *>(call.dev(mask));
         const bool sw = byteswap != 0;
         int rc = B200_OK;
         switch (dtype) {
-        case B200_F64: rc = launch_t<double>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_F32: rc = launch_t<float>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_I64: rc = launch_t<long long>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_I32: rc = launch_t<int>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_I16: rc = launch_t<short>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_I8: rc = launch_t<signed char>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_U64: rc = launch_t<unsigned long long>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_U32: rc = launch_t<unsigned>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        case B200_U16: rc = launch_t<unsigned short>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break;
-        default: rc = launch_t<unsigned char>(ctx->sm_count, sl->stream, dd, dm, nrows, sw, d); break; // uint8, bool (0 / 1)
+        case B200_F64: rc = launch_t<double>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_F32: rc = launch_t<float>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_I64: rc = launch_t<long long>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_I32: rc = launch_t<int>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_I16: rc = launch_t<short>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_I8: rc = launch_t<signed char>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_U64: rc = launch_t<unsigned long long>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_U32: rc = launch_t<unsigned>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        case B200_U16: rc = launch_t<unsigned short>(ctx->sm_count, st, dd, dm, nrows, sw, d); break;
+        default: rc = launch_t<unsigned char>(ctx->sm_count, st, dd, dm, nrows, sw, d); break; // uint8, bool (0 / 1)
         }
         B200_CHECK(rc);
     }
-    B200_CUDA(cudaMemcpyAsync(out, d, sizeof init, cudaMemcpyDeviceToHost, sl->stream));
-    B200_CUDA(cudaStreamSynchronize(sl->stream));
-    return B200_OK;
+    return call.finish();
 }

@@ -244,11 +244,12 @@ using namespace b200;
 
 extern "C" int b200_grid_mutual_information(b200_ctx *ctx, int slot, const int64_t *grid, int ndim, const int64_t *sizes, int dimension,
                                             int memspace_out, double *out) {
-    if (!ctx || slot < 0 || slot >= ctx->nslots || !grid || !sizes || dimension < 1 || ndim < dimension || ndim > B200_MAX_BINNERS ||
-        (memspace_out != B200_MEM_HOST && memspace_out != B200_MEM_DEVICE)) {
+    if (!grid || !sizes || dimension < 1 || ndim < dimension || ndim > B200_MAX_BINNERS || (memspace_out != B200_MEM_HOST && memspace_out != B200_MEM_DEVICE)) {
         set_error("b200_grid_mutual_information: invalid argument");
         return B200_ERR_INVALID;
     }
+    CallFrame call(ctx, slot, B200_MEM_DEVICE, 0, "b200_grid_mutual_information");
+    B200_CHECK(call.rc);
     MiArgs a = {};
     a.grid = reinterpret_cast<const long long *>(grid);
     a.d = dimension;
@@ -285,21 +286,8 @@ extern "C" int b200_grid_mutual_information(b200_ctx *ctx, int slot, const int64
         set_error("b200_grid_mutual_information: invalid argument (out is null)");
         return B200_ERR_INVALID;
     }
-    B200_CUDA(cudaSetDevice(ctx->device));
     B200_CHECK(b200_ctx_sync(ctx, -1)); // the grid may have been written on any slot
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    cudaStream_t st = sl->stream;
-    const size_t bytes = (size_t)a.cells * sizeof(double);
-    DevBuf<double> host_out;
-    a.out = out;
-    if (memspace_out == B200_MEM_HOST) {
-        B200_CHECK(host_out.alloc(ctx, bytes, "b200_grid_mutual_information", st));
-        a.out = host_out;
-    }
-    B200_CHECK(launch(ctx, a, st));
-    if (memspace_out == B200_MEM_HOST)
-        B200_CUDA(cudaMemcpyAsync(out, host_out, bytes, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    return B200_OK;
+    B200_CHECK(call.out(out, (size_t)a.cells * sizeof(double), memspace_out == B200_MEM_DEVICE, &a.out));
+    B200_CHECK(launch(ctx, a, call.st));
+    return call.finish(true);
 }

@@ -261,11 +261,13 @@ using namespace b200;
 
 extern "C" int b200_grid_percentile(b200_ctx *ctx, int slot, const int64_t *grid, int ndim, const int64_t *sizes, double lb, double span,
                                     const double *pct, const uint8_t *integral, int npct, int memspace_out, double *out) {
-    if (!ctx || slot < 0 || slot >= ctx->nslots || !grid || !sizes || ndim < 1 || ndim > B200_MAX_BINNERS || npct < 0 || (npct && (!pct || !integral)) ||
+    if (!grid || !sizes || ndim < 1 || ndim > B200_MAX_BINNERS || npct < 0 || (npct && (!pct || !integral)) ||
         (memspace_out != B200_MEM_HOST && memspace_out != B200_MEM_DEVICE)) {
         set_error("b200_grid_percentile: invalid argument");
         return B200_ERR_INVALID;
     }
+    CallFrame call(ctx, slot, B200_MEM_DEVICE, 0, "b200_grid_percentile");
+    B200_CHECK(call.rc);
     PctArgs a = {};
     a.grid = reinterpret_cast<const long long *>(grid);
     a.ndim = ndim - 1;
@@ -296,18 +298,10 @@ extern "C" int b200_grid_percentile(b200_ctx *ctx, int slot, const int64_t *grid
         set_error("b200_grid_percentile: invalid argument (out is null)");
         return B200_ERR_INVALID;
     }
-    B200_CUDA(cudaSetDevice(ctx->device));
     B200_CHECK(b200_ctx_sync(ctx, -1)); // the grid may have been written on any slot
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    cudaStream_t st = sl->stream;
-    const size_t bytes = (size_t)a.cells * npct * sizeof(double);
-    double *dout = out;
-    DevBuf<double> host_out;
-    if (memspace_out == B200_MEM_HOST) {
-        B200_CHECK(host_out.alloc(ctx, bytes, "b200_grid_percentile", st));
-        dout = host_out;
-    }
+    cudaStream_t st = call.st;
+    double *dout;
+    B200_CHECK(call.out(out, (size_t)a.cells * npct * sizeof(double), memspace_out == B200_MEM_DEVICE, &dout));
     for (int k0 = 0; k0 < npct; k0 += kPctMax) {
         a.npct = std::min(kPctMax, npct - k0);
         for (int k = 0; k < a.npct; k++) {
@@ -317,8 +311,5 @@ extern "C" int b200_grid_percentile(b200_ctx *ctx, int slot, const int64_t *grid
         a.out = dout + (size_t)k0 * a.cells;
         B200_CHECK(launch(a, ctx->sm_count, st));
     }
-    if (memspace_out == B200_MEM_HOST)
-        B200_CUDA(cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, st));
-    B200_CUDA(cudaStreamSynchronize(st));
-    return B200_OK;
+    return call.finish(true);
 }

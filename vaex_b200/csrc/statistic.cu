@@ -654,11 +654,12 @@ int b200_stat_reset(b200_stat *s) {
 
 int b200_stat_bin(b200_stat *s, int slot, const b200_stat_column *binby, const b200_stat_column *weights, const uint8_t *const *selections,
                   int64_t nrows, int64_t row_offset, int memspace, uint32_t flags) {
-    if (!s || slot < 0 || slot >= s->ctx->nslots || nrows < 0 || (s->ndim && !binby) || (s->nw && !weights) || memspace < B200_MEM_HOST ||
-        memspace > B200_MEM_MIXED) {
+    if (!s || nrows < 0 || (s->ndim && !binby) || (s->nw && !weights)) {
         set_error("b200_stat_bin: invalid argument");
         return B200_ERR_INVALID;
     }
+    CallFrame call(s->ctx, slot, memspace, flags, "b200_stat_bin");
+    B200_CHECK(call.rc);
     for (int i = 0; i < s->ndim + s->nw; i++) {
         const b200_stat_column &c = i < s->ndim ? binby[i] : weights[i - s->ndim];
         if (c.dtype < 0 || c.dtype >= B200_NDTYPE || (nrows && !c.data)) {
@@ -669,28 +670,23 @@ int b200_stat_bin(b200_stat *s, int slot, const b200_stat_column *binby, const b
     if (nrows == 0)
         return B200_OK;
     b200_ctx *ctx = s->ctx;
-    B200_CUDA(cudaSetDevice(ctx->device));
-    Slot *sl = ctx->slots[slot];
-    std::lock_guard<std::mutex> guard(sl->mu);
-    cudaStream_t st = sl->stream;
-    Stager stg{ctx, sl, memspace};
-    stg.async_host = (flags & B200_FLAG_ASYNC_HOST) != 0;
+    cudaStream_t st = call.st;
     for (int i = 0; i < s->ndim + s->nw; i++) {
         const b200_stat_column &c = i < s->ndim ? binby[i] : weights[i - s->ndim];
-        stg.plan(c.data, (size_t)nrows * dtype_size(c.dtype));
+        call.plan(c.data, (size_t)nrows * dtype_size(c.dtype));
         if (c.mask)
-            stg.plan(c.mask, (size_t)nrows);
+            call.plan(c.mask, (size_t)nrows);
     }
     for (int k = 0; selections && k < s->nsel; k++)
         if (selections[k])
-            stg.plan(selections[k], (size_t)nrows);
-    B200_CHECK(stg.commit());
+            call.plan(selections[k], (size_t)nrows);
+    B200_CHECK(call.commit());
 
     StatParams p;
     memset(&p, 0, sizeof p);
     bool vec = true;
     auto dev = [&](const void *h) {
-        const void *d = stg.dev(h);
+        const void *d = call.dev(h);
         if (d && (reinterpret_cast<uintptr_t>(d) & 15))
             vec = false;
         return d;
@@ -737,9 +733,7 @@ int b200_stat_bin(b200_stat *s, int slot, const b200_stat_column *binby, const b
         rc = s->cls == B200_F64 ? launch_class<double>(ctx, st, p, s->op, strat) : launch_class<float>(ctx, st, p, s->op, strat);
         B200_CHECK(rc);
     }
-    if (memspace == B200_MEM_MIXED && !(flags & B200_FLAG_ASYNC_HOST))
-        B200_CUDA(cudaStreamSynchronize(st)); // MIXED copies straight from the caller's host buffers (see b200_bin)
-    return B200_OK;
+    return call.finish();
 }
 
 int b200_stat_read(b200_stat *s, double *out) {

@@ -15,15 +15,14 @@ struct StrInput {
 };
 
 // phase 1: read offsets[0] and offsets[nrows] (a short synchronous copy when the offsets live on the device) and plan the three
-// columns on `stg`; the byte column is planned as the range the call uses, so a sliced arrow array stages only its own bytes
-inline int plan_strings(Slot *sl, Stager &stg, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, int memspace,
-                        StrInput *in) {
+// columns on `call`; the byte column is planned as the range the call uses, so a sliced arrow array stages only its own bytes
+inline int plan_strings(CallFrame &call, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, StrInput *in) {
     long long first = 0, last = 0;
     if (nrows) {
-        if (memspace == B200_MEM_DEVICE || (memspace == B200_MEM_MIXED && is_device_pointer(offsets))) {
-            B200_CUDA(cudaMemcpyAsync(&first, offsets, 8, cudaMemcpyDeviceToHost, sl->stream));
-            B200_CUDA(cudaMemcpyAsync(&last, offsets + nrows, 8, cudaMemcpyDeviceToHost, sl->stream));
-            B200_CUDA(cudaStreamSynchronize(sl->stream));
+        if (call.on_device(offsets)) {
+            B200_CUDA(cudaMemcpyAsync(&first, offsets, 8, cudaMemcpyDeviceToHost, call.st));
+            B200_CUDA(cudaMemcpyAsync(&last, offsets + nrows, 8, cudaMemcpyDeviceToHost, call.st));
+            B200_CUDA(cudaStreamSynchronize(call.st));
         } else {
             first = offsets[0], last = offsets[nrows];
         }
@@ -34,28 +33,27 @@ inline int plan_strings(Slot *sl, Stager &stg, const int64_t *offsets, const uin
     }
     in->base = first;
     in->nbytes = last - first;
-    stg.plan(offsets, (size_t)(nrows + 1) * 8);
+    call.plan(offsets, (size_t)(nrows + 1) * 8);
     if (in->nbytes)
-        stg.plan(bytes + first, (size_t)in->nbytes);
+        call.plan(bytes + first, (size_t)in->nbytes);
     if (masks)
-        stg.plan(masks, (size_t)nrows);
+        call.plan(masks, (size_t)nrows);
     return B200_OK;
 }
 
-// phase 2, after stg.commit(): the device pointers.  Device columns are used in place (Stager::dev returns them unchanged), so
+// phase 2, after call.commit(): the device pointers.  Device columns are used in place (CallFrame::dev returns them unchanged), so
 // `bytes` + base is the row range's first byte in every memspace.
-inline void resolve_strings(const Stager &stg, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, StrInput *in) {
-    in->offsets = static_cast<const long long *>(stg.dev(offsets));
-    in->bytes = in->nbytes ? static_cast<const unsigned char *>(stg.dev(bytes + in->base)) : bytes;
-    in->masks = masks ? static_cast<const uint8_t *>(stg.dev(masks)) : nullptr;
+inline void resolve_strings(const CallFrame &call, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, StrInput *in) {
+    in->offsets = static_cast<const long long *>(call.dev(offsets));
+    in->bytes = in->nbytes ? static_cast<const unsigned char *>(call.dev(bytes + in->base)) : bytes;
+    in->masks = masks ? static_cast<const uint8_t *>(call.dev(masks)) : nullptr;
 }
 
 // both phases for a call that stages nothing else
-inline int stage_strings(Slot *sl, Stager &stg, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, int memspace,
-                         StrInput *in) {
-    B200_CHECK(plan_strings(sl, stg, offsets, bytes, masks, nrows, memspace, in));
-    B200_CHECK(stg.commit());
-    resolve_strings(stg, offsets, bytes, masks, in);
+inline int stage_strings(CallFrame &call, const int64_t *offsets, const uint8_t *bytes, const uint8_t *masks, int64_t nrows, StrInput *in) {
+    B200_CHECK(plan_strings(call, offsets, bytes, masks, nrows, in));
+    B200_CHECK(call.commit());
+    resolve_strings(call, offsets, bytes, masks, in);
     return B200_OK;
 }
 

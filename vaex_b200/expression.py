@@ -360,19 +360,17 @@ class DeviceExpression:
             return out
         nin = len(self.columns)
         inputs = (_lib.ExprInput * max(nin, 1))()
-        keep, spaces = [], set()
+        keep = []
         for k, col in enumerate(self.columns):
             part = col[i1:i2]
             if isinstance(part, np.ndarray) and not part.dtype.isnative:
                 part = part.astype(part.dtype.newbyteorder("="))
             c = _lib.column(part)
             keep.append(c)
-            spaces.add(c.memspace)
             inputs[k].data, inputs[k].dtype = c.ptr, c.code
         sets = (C.c_void_p * max(len(self.program.sets), 1))(*[s._h for s in self.program.sets])
-        memspace = _lib.MEM_HOST if spaces == {_lib.MEM_HOST} else _lib.MEM_DEVICE if spaces <= {_lib.MEM_DEVICE} else _lib.MEM_MIXED
         _lib.check(_lib.lib().b200_eval(self._ctx._h, self._ctx.slot(thread_index), self._ops, len(self.program.ops), inputs, nin, sets, len(self.program.sets), n,
-                                        memspace, _lib.DTYPE_CODE[self.dtype.name], raw.data_ptr()))
+                                        _lib.memspace(*keep), _lib.DTYPE_CODE[self.dtype.name], raw.data_ptr()))
         return out
 
     def evaluate(self, i1=0, i2=None, thread_index=0):
@@ -423,7 +421,5 @@ def compact(thread_index, keep_mask, columns, ctx=None):
     optr = (C.c_void_p * max(ncols, 1))(*[b.data_ptr() for b in bufs])
     dts = (C.c_int32 * max(ncols, 1))(*[c.code for c in cols])
     count = C.c_int64(0)
-    spaces = {c.memspace for c in cols} | {km.memspace}
-    memspace = _lib.MEM_HOST if spaces == {_lib.MEM_HOST} else _lib.MEM_DEVICE if spaces == {_lib.MEM_DEVICE} else _lib.MEM_MIXED
-    _lib.check(_lib.lib().b200_compact(ctx._h, ctx.slot(thread_index), km.ptr, ncols, cptr, dts, n, memspace, optr, C.byref(count)))
+    _lib.check(_lib.lib().b200_compact(ctx._h, ctx.slot(thread_index), km.ptr, ncols, cptr, dts, n, _lib.memspace(km, *cols), optr, C.byref(count)))
     return count.value, [DeviceArray(b.data_ptr(), count.value, c.dtype, keep=b) for b, c in zip(bufs, cols)]

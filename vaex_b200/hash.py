@@ -247,7 +247,7 @@ class CombinedCodes:
         if n == 0:
             return out
         nk = len(self.columns)
-        keep, kptr, mptr, spaces = [], (C.c_void_p * nk)(), (C.c_void_p * nk)(), set()
+        keep, kptr, mptr = [], (C.c_void_p * nk)(), (C.c_void_p * nk)()
         for k, col in enumerate(self.columns):
             # a previous stage's codes (vaex/groupby.py:572-582) are produced on this worker's slot, like every device-virtual column
             part = col.chunk(thread_index, i1, i2) if getattr(col, "device_virtual", False) else col[i1:i2]
@@ -261,7 +261,6 @@ class CombinedCodes:
             if c.dtype.itemsize != self.hash_maps[k].dtype.itemsize:
                 raise RuntimeError("stride not equal to bytesize for key values")
             keep.append(c)
-            spaces.add(c.memspace)
             kptr[k] = c.ptr
             if mask is not None:
                 m = _lib.mask_column(mask)
@@ -269,8 +268,8 @@ class CombinedCodes:
                 mptr[k] = m.ptr
         sets = (C.c_void_p * nk)(*[hm._internal._h for hm in self.hash_maps])
         mult = (C.c_int64 * nk)(*self.multipliers)
-        memspace = _lib.MEM_DEVICE if spaces == {_lib.MEM_DEVICE} else _lib.MEM_MIXED
-        _lib.check(_lib.lib().b200_set_combine(self._ctx._h, self._ctx.slot(thread_index), nk, sets, kptr, mptr, mult, n, out.data_ptr(), memspace, 0))
+        _lib.check(_lib.lib().b200_set_combine(self._ctx._h, self._ctx.slot(thread_index), nk, sets, kptr, mptr, mult, n, out.data_ptr(),
+                                               _lib.memspace(*keep), 0))
         return out
 
     def decode(self, codes):

@@ -128,7 +128,7 @@ class Statistic:
     def bin(self, slot, binby, weights, selections, nrows, row_offset):
         """binby / weights: arrays (numpy, numpy.ma or device); selections: one entry per selection, None = all rows.
         row_offset: the global index of the block's first row; FIRST breaks ties by it, so every row of a pass needs its own."""
-        keep, spaces = [], set()
+        keep = []
 
         def column(ar):
             mask = None
@@ -142,9 +142,6 @@ class Statistic:
             if c.length != nrows:
                 raise RuntimeError(f"expected a block of {nrows} rows, got {c.length}")
             keep.extend([c, mask])
-            spaces.add(c.memspace)
-            if mask is not None:
-                spaces.add(mask.memspace)
             return StatColumn(c.ptr, c.code, c.byteswap, None if mask is None else mask.ptr)
 
         b = (StatColumn * max(len(binby), 1))(*[column(a) for a in binby])
@@ -154,9 +151,8 @@ class Statistic:
             if s is not None:
                 m = _lib.mask_column(s)
                 keep.append(m)
-                spaces.add(m.memspace)
                 sel[i] = m.ptr
-        memspace = spaces.pop() if len(spaces) == 1 else (_lib.MEM_MIXED if spaces else _lib.MEM_HOST)
+        memspace = _lib.memspace(*keep)
         slot = self.ctx.slot(0 if slot is None else slot)
         if self._held.pop(slot, None) is not None:
             self.ctx.sync(slot)  # the previous call's kernel on this slot is done with its blocks

@@ -237,10 +237,7 @@ class Grid:
         A = (_lib.AggInput * na)()
         for k, agg in enumerate(aggregators):
             keep += agg._fill(A[k], thread)
-        spaces = {c.memspace for c in keep}
-        # host and device columns in one call (device-computed group codes next to host value columns): every pointer is
-        # classified by the library
-        memspace = _lib.MEM_MIXED if len(spaces) > 1 else (spaces.pop() if spaces else _lib.MEM_HOST)
+        memspace = _lib.memspace(*keep)
         for c in keep:
             if c.length < length:
                 raise RuntimeError(f"a column of length {c.length} is shorter than the {length} rows to bin")

@@ -108,8 +108,7 @@ class _OrderedSet:
         out_values = np.empty(n if rv else 1, np.int64)
         out_map = np.empty(n if rv else 1, np.int16)
         _lib.check(_lib.lib().b200_set_update(self._h, 0, col.ptr, None if mcol is None else mcol.ptr, n, int(opts["start_index"]), int(rv),
-                                              out_values.ctypes.data, out_map.ctypes.data,
-                                              col.memspace if mcol is None or mcol.memspace == col.memspace else _lib.MEM_MIXED, 0))
+                                              out_values.ctypes.data, out_map.ctypes.data, _lib.memspace(col, mcol), 0))
         if rv:
             return out_values, out_map
         return None
