@@ -287,6 +287,22 @@ int b200_stat_fields(const b200_stat *stat);
 int b200_stat_read(b200_stat *stat, double *out);
 int b200_stat_reset(b200_stat *stat);
 int b200_stat_destroy(b200_stat *stat);
+/* df.mode's count and finish (vaex/dataframe.py:2006-2034): vaex.legacy.TaskHistogram (vaex/legacy.py:22-110) over vaexfast
+ * histogram2d / histogram3d / histogramNd (src/vaexfast.cpp:577-600, 818-860, 939-965).  b200_stat_create_histogram makes an ADD1
+ * statistic of class B200_F64 with one selection whose grid is the reference's histogram grid: `sizes`, `minima` and `maxima` in
+ * grid axis order, axis 0 slowest.  vaexfast bins its first block along the LAST axis, so the caller passes the reference's blocks
+ * reversed (mode: the expression on axis 0, the first binby on the last axis).  Two dimensions bin like histogram2d (= statisticNd
+ * of class double; a non-finite limit counts nothing), three or more like histogram3d / histogramNd (min <= v < max, bin
+ * (int)((v-min) * (size/(max-min)))); more than three need equal sizes (B200_ERR_UNSUPPORTED otherwise: histogramNd strides by
+ * the reversed axis but scales by the unreversed one).  A bin that rounds up to `size` lands in the last bin and a NaN bin (an
+ * infinite minimum) drops the row, where the reference writes outside its grid.  Masks are read (use NULL to bin the values under
+ * a mask, as vaexfast does); b200_stat_bin / read / reset / destroy work as for any statistic.
+ * b200_stat_mode: the argmax finish.  For every cell of axes 1.. (C order) out[cell] = centers[the first index of the largest count
+ * along axis 0], or NaN when the cell's counts are all zero; `centers` holds sizes[0] doubles, `out` the product of the other
+ * sizes, both host memory.  Like b200_stat_read it is not a per-slot call: it waits for every slot, runs on slot 0's stream under
+ * that slot's lock, and returns when `out` is written; only `out` is copied back, never the grid. */
+int b200_stat_create_histogram(b200_ctx *ctx, int ndim, const int64_t *sizes, const double *minima, const double *maxima, b200_stat **out);
+int b200_stat_mode(b200_stat *stat, const double *centers, double *out);
 
 /* ---- percentile_approx / median_approx: the finish of a count grid (vaex/dataframe.py:1675-1754) ----------------------------
  * `grid` is a DEVICE int64 count grid with edges, first dimension fastest: the binby dimensions, then the percentile axis last,

@@ -2,7 +2,7 @@
 """Times every BASELINE.json configuration on one H100 with device-resident columns (the roofline setting) and prints one
 JSON object per config: rows/s, achieved algorithmic GB/s (SURVEY.md 8d bytes/row) and the fraction of the measured HBM peak.
 
-    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV,PA,MI]
+    python tools/bench_configs.py [--rows 1e9] [--configs C1,C2,C3,C4,C5,CV,PA,MI,MO]
 
 This is a companion to bench.py (which owns the headline line the driver parses); results are quoted in DESIGN.md.
 """
@@ -237,6 +237,8 @@ def main():
             pa_percentile(args, n, ctx, stream, gen, timed, report)
         elif cfg == "MI":
             mi_mutual_information(args, n, ctx, stream, gen, timed, report)
+        elif cfg == "MO":
+            mo_mode(args, n, ctx, stream, gen, timed, report)
 
 
 def pa_percentile(args, n, ctx, stream, gen, timed, report):
@@ -375,6 +377,66 @@ def mi_mutual_information(args, n, ctx, stream, gen, timed, report):
                           "column), 36 count grids in one pass, 36 device finishes", rows=n, ms=best, parity=ok, gpu=power)), flush=True)
     print(json.dumps(dict(config="MI", parity=bool(parity), gpu=power)), flush=True)
     del f, cols, x, y, z
+
+
+def mo_mode(args, n, ctx, stream, gen, timed, report):
+    """MO: df.mode(v, binby, mode_shape=64, mode_limits=[-4, 4]) over `n` device-resident fp32 rows, (a) binby=[x] shape 256 (a 64 x 256
+    grid: the shared-memory count) and (b) binby=[x, y] shape 256 (64 x 256^2 = 4M cells, 32 MB: the global count), limits [-3, 3].
+    Timed separately with CUDA events: the count pass and the device finish (b200_stat_mode, which includes copying the modes back).
+    Beside them the host finish the reference runs: the D2H of the count grid and numpy's argmax finish (tests/mode_oracle.finish).
+    Parity: the device histogram and finish of the first 2^22 rows against the numpy restatement of those rows, bit for bit."""
+    import subprocess
+    import numpy as np
+    import torch
+    from vaex_b200 import mode as _mode
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import mode_oracle as MO
+    from helpers import same_bits
+    power = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    x, y, v = (torch.empty(n, dtype=torch.float32, device="cuda").normal_(generator=gen) for _ in range(3))
+    centers = _mode.centers(-4.0, 4.0, 64)
+    sub = 1 << 22
+    parity = True
+    for name, binby in (("MO-1d", [x]), ("MO-2d", [x, y])):
+        shape = (64,) + (256,) * len(binby)
+        blocks = binby + [v]
+        lims = [(-3.0, 3.0)] * len(binby) + [(-4.0, 4.0)]
+        order, olims = _mode.axis_order(blocks), _mode.axis_order(lims)
+        h = _mode.Histogram(shape, [lo for lo, _ in olims], [hi for _, hi in olims], ctx=ctx)
+        small = _mode.Histogram(shape, [lo for lo, _ in olims], [hi for _, hi in olims], ctx=ctx)
+        small.bin(0, [c[:sub] for c in order], [], [None], sub, 0)
+        got = small.mode(centers)
+        small.close()
+        want = MO.finish(MO.histogram([c[:sub].cpu().numpy() for c in blocks], lims, shape), -4.0, 4.0, 64)
+        ok = same_bits(got, want)
+        parity &= ok
+
+        def count():
+            h.bin(0, order, [], [None], n, 0)
+        ms_count = timed(count, args.reps, setup=h.reset)
+        ms_finish = timed(lambda: h.mode(centers), args.reps)
+        host_best = d2h_best = None
+        for _ in range(max(2, args.reps // 2)):
+            t0 = time.perf_counter()
+            grid = h.read()  # D2H into pageable memory
+            t1 = time.perf_counter()
+            MO.finish(grid, -4.0, 4.0, 64)
+            t2 = time.perf_counter()
+            d2h_best = min(d2h_best or 1e30, (t1 - t0) * 1e3)
+            host_best = min(host_best or 1e30, (t2 - t0) * 1e3)
+        assert int(grid.sum()) <= n
+        workload = f"mode(v, binby=[{', '.join('xy'[:len(binby)])}], shape=256, mode_shape=64) on fp32 rows"
+        report(name + "/count", workload + ": count pass", n, 4 * len(blocks), ms_count,
+               kernel="k_stat_count_smem" if np.prod(shape) * 4 <= 96 * 1024 else "k_stat_global", gpu=power)
+        print(json.dumps(dict(config=name + "/finish", workload=workload + ": argmax finish on the device, modes copied back", ms=ms_finish,
+                              grid_bytes=8 * int(np.prod(shape)), parity=ok, gpu=power)), flush=True)
+        print(json.dumps(dict(config=name + "/host_finish", workload=workload + ": D2H (pageable) + numpy finish on the host", ms=host_best,
+                              d2h_ms=d2h_best, gpu=power)), flush=True)
+        h.close()
+        del h, grid
+        torch.cuda.empty_cache()
+    print(json.dumps(dict(config="MO", parity=bool(parity), gpu=power)), flush=True)
+    del x, y, v
 
 
 def ls_string_list(args, ctx, stream, gen, report):

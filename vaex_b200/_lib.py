@@ -162,6 +162,8 @@ def lib():
             "b200_stat_read": (i32, [vp, vp]),
             "b200_stat_reset": (i32, [vp]),
             "b200_stat_destroy": (i32, [vp]),
+            "b200_stat_create_histogram": (i32, [vp, i32, P(i64), P(C.c_double), P(C.c_double), P(vp)]),
+            "b200_stat_mode": (i32, [vp, vp, vp]),
             "b200_grid_percentile": (i32, [vp, i32, vp, i32, P(i64), C.c_double, C.c_double, P(C.c_double), P(C.c_uint8), i32, i32, vp]),
             "b200_grid_mutual_information": (i32, [vp, i32, vp, i32, P(i64), i32, i32, vp]),
             "b200_host_register": (i32, [vp, sz]),

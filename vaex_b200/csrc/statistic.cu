@@ -18,7 +18,16 @@
 //   k_stat_smem   the whole (selections x cells x fields) accumulator fits in shared memory: a block-private copy, flushed once;
 //   k_stat_global otherwise: atomics on the device accumulator.
 // FIRST always runs k_stat_first<T, false> (select) + k_stat_first<T, true> (deposit) on the device accumulator.
+//
+// df.mode's count (vaex/dataframe.py:2006-2034 -> vaex.legacy.TaskHistogram, vaex/legacy.py:22-110 -> vaexfast histogram2d /
+// histogram3d / histogramNd, src/vaexfast.cpp:577-600, 818-860, 939-965) is an ADD1 grid of class double built by
+// b200_stat_create_histogram.  Two dimensions bin exactly like statisticNd of class double without edges, so they run the statistic
+// rule; three or more run the kBinHist rule of histogram3d / histogramNd: a row is kept when min <= v < max and its bin is
+// (int)((v-min)*scale) with scale = size/(max-min).  A bin index that rounds up to `size` goes to the last bin, as statisticNd's
+// does, and a NaN index (an infinite minimum) drops the row.  Histograms whose 32-bit counts fit shared memory run k_stat_count_smem,
+// the others k_stat_global; k_stat_mode is the per-cell argmax finish.
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 #include "cas128.cuh"
@@ -29,6 +38,9 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr size_t kSmemBudget = 96 * 1024;
+constexpr size_t kSmemPerSm = 200 * 1024; // of an H100 SM's 228 KB, what the histogram count's CTAs share
+
+enum BinRule { kBinStat, kBinHist }; // statisticNd's bins, or histogram3d / histogramNd's
 
 struct StatCol {
     const void *data;
@@ -40,7 +52,7 @@ struct StatParams {
     StatCol bin[B200_MAX_BINNERS];
     StatCol w[B200_STAT_MAX_WEIGHTS];
     const uint8_t *sel[B200_STAT_MAX_SELECTIONS]; // non-zero = keep; NULL = all rows
-    double minv[B200_MAX_BINNERS], scale[B200_MAX_BINNERS]; // values of class T
+    double minv[B200_MAX_BINNERS], maxv[B200_MAX_BINNERS], scale[B200_MAX_BINNERS]; // values of class T
     int size[B200_MAX_BINNERS];
     long long stride[B200_MAX_BINNERS]; // in cells
     int ndim, nw, nsel, edges, vec;
@@ -74,10 +86,20 @@ __device__ __forceinline__ int trunc_int(T a) {
         return __float2int_rz(a);
 }
 
-// statisticNd's bin of one value along dimension d; -1 = outside (no edges)
-template <typename T>
+// statisticNd's (or, kBinHist, histogram3d / histogramNd's) bin of one value along dimension d; -1 = outside (no edges)
+template <typename T, int RULE>
 __device__ __forceinline__ int stat_bin(const StatParams &p, int d, T v) {
     const int size = p.size[d];
+    if constexpr (RULE == kBinHist) {
+        if (!(v >= (T)p.minv[d] && v < (T)p.maxv[d]))
+            return -1;
+        const T f = mul_rn<T>(sub_rn<T>(v, (T)p.minv[d]), (T)p.scale[d]);
+        // (v-min) can round up to max-min, so f can reach `size`: the reference then writes past its row, here the row lands in
+        // the last bin.  An infinite minimum gives inf * 0 = NaN, where the reference indexes with INT_MIN: the row is dropped.
+        if (f != f)
+            return -1;
+        return min(trunc_int<T>(f), size - 1);
+    }
     const T scaled = mul_rn<T>(sub_rn<T>(v, (T)p.minv[d]), (T)p.scale[d]);
     int b;
     if (p.edges) {
@@ -141,7 +163,7 @@ __device__ __forceinline__ void drop_masked(const StatParams &p, const StatCol &
 }
 
 // flat cell of four rows and whether each takes part at all (inside the grid, unmasked in every column)
-template <typename T>
+template <typename T, int RULE>
 __device__ __forceinline__ void rows4(const StatParams &p, long long base, int nv, long long idx[4], bool ok[4]) {
 #pragma unroll
     for (int j = 0; j < 4; j++)
@@ -155,7 +177,7 @@ __device__ __forceinline__ void rows4(const StatParams &p, long long base, int n
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             const uint64_t b = p.bin[d].swap ? bswap(r[j], p.bin[d].isz) : r[j];
-            const int k = stat_bin<T>(p, d, raw_class_value<T>(p.bin[d].dt, b));
+            const int k = stat_bin<T, RULE>(p, d, raw_class_value<T>(p.bin[d].dt, b));
             ok[j] = ok[j] && k >= 0;
             idx[j] += p.stride[d] * (long long)max(k, 0);
         }
@@ -226,7 +248,7 @@ __device__ __forceinline__ void weights4(const StatParams &p, long long base, in
             load4_values<T>(p, p.w[c], base, nv, wv[c]);
 }
 
-template <typename T, int OP, int NT>
+template <typename T, int OP, int NT, int RULE>
 __device__ __forceinline__ void bin_rows_atomic(const StatParams &p, unsigned long long *acc) {
     constexpr int W = NT > 0 ? NT : 1;
     const long long step = (long long)gridDim.x * kThreads * 4;
@@ -235,7 +257,7 @@ __device__ __forceinline__ void bin_rows_atomic(const StatParams &p, unsigned lo
         const int nv = left < 4 ? (int)left : 4;
         long long idx[4];
         bool ok[4];
-        rows4<T>(p, base, nv, idx, ok);
+        rows4<T, RULE>(p, base, nv, idx, ok);
         double wv[W][4];
         if constexpr (NT > 0)
             weights4<T, NT>(p, base, nv, wv);
@@ -260,19 +282,61 @@ __device__ __forceinline__ unsigned long long init_slot(const StatParams &p, int
     return 0;
 }
 
-template <typename T, int OP, int NT>
+template <typename T, int OP, int NT, int RULE>
 __global__ void __launch_bounds__(kThreads) k_stat_global(const __grid_constant__ StatParams p) {
-    bin_rows_atomic<T, OP, NT>(p, p.acc);
+    bin_rows_atomic<T, OP, NT, RULE>(p, p.acc);
 }
 
-template <typename T, int OP, int NT>
+// the histogram's ADD1 count with one selection in a block-private grid of 32-bit counts (half the shared memory of k_stat_smem's
+// 64-bit slots, so mode's default 64 x 256 grid fits), flushed once into the 64-bit device grid.  The host picks it only when no
+// CTA can see 2^32 rows.
+template <int RULE>
+__global__ void __launch_bounds__(kThreads) k_stat_count_smem(const __grid_constant__ StatParams p) {
+    extern __shared__ unsigned scount[];
+    for (long long i = threadIdx.x; i < p.cells; i += kThreads)
+        scount[i] = 0;
+    __syncthreads();
+    const long long step = (long long)gridDim.x * kThreads * 4;
+    for (long long base = ((long long)blockIdx.x * kThreads + threadIdx.x) * 4; base < p.nrows; base += step) {
+        const long long left = p.nrows - base;
+        const int nv = left < 4 ? (int)left : 4;
+        long long idx[4];
+        bool ok[4];
+        rows4<double, RULE>(p, base, nv, idx, ok);
+#pragma unroll
+        for (int j = 0; j < 4; j++)
+            if (ok[j] && selected(p, 0, base + j))
+                atomicAdd(scount + idx[j], 1u);
+    }
+    __syncthreads();
+    for (long long i = threadIdx.x; i < p.cells; i += kThreads)
+        if (scount[i])
+            atomicAdd(p.acc + i, (unsigned long long)scount[i]);
+}
+
+// mode's finish: one thread per cell of axes 1.. walks axis 0 (coalesced across cells) and keeps its first maximum, as np.argmax;
+// an all-zero cell gives NaN
+__global__ void __launch_bounds__(kThreads) k_stat_mode(const unsigned long long *counts, int n0, long long cells, const double *centers, double *out) {
+    for (long long c = (long long)blockIdx.x * kThreads + threadIdx.x; c < cells; c += (long long)gridDim.x * kThreads) {
+        unsigned long long best = 0;
+        int at = 0;
+        for (int m = 0; m < n0; m++) {
+            const unsigned long long v = counts[(long long)m * cells + c];
+            if (v > best)
+                best = v, at = m;
+        }
+        out[c] = best ? centers[at] : __longlong_as_double(0x7ff8000000000000LL);
+    }
+}
+
+template <typename T, int OP, int NT, int RULE>
 __global__ void __launch_bounds__(kThreads) k_stat_smem(const __grid_constant__ StatParams p) {
     extern __shared__ unsigned long long sacc[];
     const long long n = (long long)p.nsel * p.cells * p.K;
     for (long long i = threadIdx.x; i < n; i += kThreads)
         sacc[i] = init_slot(p, OP, (int)(i % p.K));
     __syncthreads();
-    bin_rows_atomic<T, OP, NT>(p, sacc);
+    bin_rows_atomic<T, OP, NT, RULE>(p, sacc);
     __syncthreads();
     for (long long i = threadIdx.x; i < n; i += kThreads) {
         const unsigned long long v = sacc[i];
@@ -428,7 +492,7 @@ __global__ void __launch_bounds__(kThreads) k_stat_first(const __grid_constant__
         const int nv = left < 4 ? (int)left : 4;
         long long idx[4];
         bool ok[4];
-        rows4<T>(p, base, nv, idx, ok);
+        rows4<T, kBinStat>(p, base, nv, idx, ok);
         double wv[2][4];
         weights4<T, 2>(p, base, nv, wv);
 #pragma unroll
@@ -478,9 +542,9 @@ int launch(Kern k, b200_ctx *ctx, cudaStream_t st, const StatParams &p, int per_
     return B200_OK;
 }
 
-enum Strategy { kReg, kSmem, kGlobal, kFirst };
+enum Strategy { kReg, kSmem, kGlobal, kFirst, kCountSmem };
 
-template <typename T, int OP, int NT>
+template <typename T, int OP, int NT, int RULE = kBinStat>
 int launch_op(b200_ctx *ctx, cudaStream_t st, const StatParams &p, Strategy s) {
     const size_t bytes = (size_t)p.nsel * p.cells * p.K * 8;
     if constexpr (OP != B200_STAT_FIRST) {
@@ -488,9 +552,15 @@ int launch_op(b200_ctx *ctx, cudaStream_t st, const StatParams &p, Strategy s) {
             if constexpr (NT > 0)
                 return launch(k_stat_reg<T, OP, NT>, ctx, st, p, 8, 0);
         } else if (s == kSmem) {
-            return launch(k_stat_smem<T, OP, NT>, ctx, st, p, bytes > 48 * 1024 ? 2 : 4, bytes);
+            if constexpr (RULE == kBinStat) // histograms count in k_stat_count_smem
+                return launch(k_stat_smem<T, OP, NT, RULE>, ctx, st, p, bytes > 48 * 1024 ? 2 : 4, bytes);
+        } else if (s == kCountSmem) {
+            if constexpr (OP == B200_STAT_ADD1) {
+                const size_t sbytes = (size_t)p.cells * 4;
+                return launch(k_stat_count_smem<RULE>, ctx, st, p, (int)std::max<size_t>(1, std::min<size_t>(8, kSmemPerSm / sbytes)), sbytes);
+            }
         } else {
-            return launch(k_stat_global<T, OP, NT>, ctx, st, p, 8, 0);
+            return launch(k_stat_global<T, OP, NT, RULE>, ctx, st, p, 8, 0);
         }
     } else {
         B200_CHECK(launch(k_stat_first<T, false>, ctx, st, p, 8, 0));
@@ -541,8 +611,11 @@ struct b200_stat {
     b200_ctx *ctx = nullptr;
     int op = 0, cls = 0, ndim = 0, edges = 0, nw = 0, nsel = 0;
     int nc = 0, K = 0; // device layout per cell (see StatParams)
+    bool hist = false;   // b200_stat_create_histogram: df.mode's count
+    int rule = kBinStat; // its bin rule
+    bool empty = false;  // histogram2d with a non-finite limit counts nothing
     int64_t sizes[B200_MAX_BINNERS] = {};
-    double minv[B200_MAX_BINNERS] = {}, scale[B200_MAX_BINNERS] = {};
+    double minv[B200_MAX_BINNERS] = {}, maxv[B200_MAX_BINNERS] = {}, scale[B200_MAX_BINNERS] = {};
     long long stride[B200_MAX_BINNERS] = {};
     long long cells = 1;
     DevBuf<unsigned long long> acc;
@@ -627,6 +700,56 @@ int b200_stat_create(b200_ctx *ctx, int op, int cls, int ndim, const int64_t *si
     return B200_OK;
 }
 
+int b200_stat_create_histogram(b200_ctx *ctx, int ndim, const int64_t *sizes, const double *minima, const double *maxima, b200_stat **out) {
+    if (!ctx || !out || ndim < 2 || ndim > B200_MAX_BINNERS || !sizes || !minima || !maxima) {
+        set_error("b200_stat_create_histogram: invalid argument (2 to %d dimensions)", B200_MAX_BINNERS);
+        return B200_ERR_INVALID;
+    }
+    for (int d = 1; ndim > 3 && d < ndim; d++)
+        if (sizes[d] != sizes[0]) { // histogramNd scales block e by count_sizes[e] but strides it by axis ndim-1-e
+            set_error("b200_stat_create_histogram: %d dimensions need equal sizes (histogramNd mixes up the axes of unequal ones)", ndim);
+            return B200_ERR_UNSUPPORTED;
+        }
+    b200_stat *raw = nullptr;
+    B200_CHECK(b200_stat_create(ctx, B200_STAT_ADD1, B200_F64, ndim, sizes, minima, maxima, 0, 0, 1, &raw));
+    raw->hist = true;
+    raw->rule = ndim == 2 ? kBinStat : kBinHist;
+    for (int d = 0; d < ndim; d++) {
+        raw->maxv[d] = maxima[d];
+        raw->empty |= ndim == 2 && !(std::isfinite(minima[d]) && std::isfinite(maxima[d])); // src/vaexfast.cpp:582-583
+        if (ndim > 2) {
+            volatile double diff = maxima[d] - minima[d]; // histogram3d / histogramNd: scale = size / (max - min)
+            raw->scale[d] = (double)sizes[d] / diff;
+        }
+    }
+    *out = raw;
+    return B200_OK;
+}
+
+int b200_stat_mode(b200_stat *s, const double *centers, double *out) {
+    if (!s || !s->hist || !centers || !out) {
+        set_error("b200_stat_mode: invalid argument (a histogram of b200_stat_create_histogram, centers and out)");
+        return B200_ERR_INVALID;
+    }
+    b200_ctx *ctx = s->ctx;
+    B200_CUDA(cudaSetDevice(ctx->device));
+    B200_CHECK(b200_ctx_sync(ctx, -1)); // the grid may have been written on any slot
+    Slot *sl = ctx->slots[0];
+    std::lock_guard<std::mutex> lock(sl->mu);
+    cudaStream_t st = sl->stream;
+    const int n0 = (int)s->sizes[0];
+    const long long cells = s->cells / n0;
+    DevBuf<double> dev;
+    B200_CHECK(dev.alloc(ctx, (size_t)(n0 + cells) * sizeof(double), "b200_stat_mode", st));
+    B200_CUDA(cudaMemcpyAsync(dev, centers, (size_t)n0 * sizeof(double), cudaMemcpyHostToDevice, st));
+    const long long blocks = std::max<long long>(1, std::min<long long>((cells + kThreads - 1) / kThreads, (long long)ctx->sm_count * 8));
+    k_stat_mode<<<(unsigned)blocks, kThreads, 0, st>>>(s->acc, n0, cells, dev, dev + n0);
+    B200_CUDA(cudaGetLastError());
+    B200_CUDA(cudaMemcpyAsync(out, dev + n0, (size_t)cells * sizeof(double), cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    return B200_OK;
+}
+
 int b200_stat_destroy(b200_stat *s) {
     if (!s)
         return B200_OK;
@@ -667,7 +790,7 @@ int b200_stat_bin(b200_stat *s, int slot, const b200_stat_column *binby, const b
             return B200_ERR_INVALID;
         }
     }
-    if (nrows == 0)
+    if (nrows == 0 || s->empty)
         return B200_OK;
     b200_ctx *ctx = s->ctx;
     cudaStream_t st = call.st;
@@ -702,7 +825,7 @@ int b200_stat_bin(b200_stat *s, int slot, const b200_stat_column *binby, const b
     };
     for (int d = 0; d < s->ndim; d++) {
         p.bin[d] = col(binby[d]);
-        p.minv[d] = s->minv[d], p.scale[d] = s->scale[d], p.size[d] = (int)s->sizes[d], p.stride[d] = s->stride[d];
+        p.minv[d] = s->minv[d], p.maxv[d] = s->maxv[d], p.scale[d] = s->scale[d], p.size[d] = (int)s->sizes[d], p.stride[d] = s->stride[d];
     }
     for (int k = 0; k < s->nw; k++)
         p.w[k] = col(weights[k]);
@@ -714,6 +837,13 @@ int b200_stat_bin(b200_stat *s, int slot, const b200_stat_column *binby, const b
     p.acc = s->acc;
 
     Strategy strat;
+    if (s->hist) {
+        strat = (size_t)s->cells * 4 <= kSmemBudget && nrows < (1LL << 32) ? kCountSmem : kGlobal;
+        const int rc = s->rule == kBinHist ? launch_op<double, B200_STAT_ADD1, 2, kBinHist>(ctx, st, p, strat)
+                                           : launch_op<double, B200_STAT_ADD1, 2, kBinStat>(ctx, st, p, strat);
+        B200_CHECK(rc);
+        return call.finish();
+    }
     if (s->op == B200_STAT_FIRST)
         strat = kFirst;
     else if (s->ndim == 0 && s->nsel == 1 && (s->op != B200_STAT_COV || s->nw <= 4))

@@ -446,6 +446,42 @@ class Frame:
             del tasks, part  # the batch's count grids go back before the next batch allocates
         return _mi.assemble(mi_list, x, unique_reverse, binby_shape, shape_result, waslist, sort)
 
+    # ---- mode: the legacy histogram counted on the device, the argmax finish on the device (csrc/statistic.cu) ---------------
+    def mode(self, expression, binby=[], limits=None, shape=256, mode_shape=64, mode_limits=None, selection=None):
+        """df.mode (vaex/dataframe.py:2006-2034): per cell of the binby grid the center of the `mode_shape`-bin histogram bin of
+        `expression` that holds the most rows (the first such bin), NaN where the cell is empty.  The histogram is vaex's legacy one
+        (vaexfast histogram2d / 3d / Nd with their own bin rules, DESIGN.md section 3): the result is indexed with the LAST binby
+        first, and with three binby every size must equal `mode_shape`.  `limits` / `mode_limits` are pairs, "minmax" / None or
+        "N%"; `selection` is a boolean expression whose rows are counted.  A string `binby` is one expression."""
+        from . import mode as _mode
+        binby = [str(b) for b in ([binby] if isinstance(binby, str) else list(binby))]
+        expression = str(expression)
+        shape = _mode.grid_shape(binby, shape, mode_shape)
+        selection = None if selection is False else selection
+        f = self
+        names = list(dict.fromkeys(binby + [expression]))
+        missing = [e for e in names if e not in self.columns]
+        if missing:
+            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
+            for e in missing:
+                f.columns[e] = f.expression(e)
+        for e in names:
+            if _dtype_of(f.columns[e]).kind not in "biuf":
+                raise NotImplementedError(f"mode over the string, object or datetime column {e!r} is not supported")
+        limits = list(f.limits(binby, limits)) + list(f.limits([expression], mode_limits))
+        centers = _mode.centers(*limits[-1], mode_shape)
+        _mode.check_memory(shape, _lib.context().device)
+        mask = f.expression(selection) if isinstance(selection, str) else selection
+        if isinstance(selection, str) and mask.dtype != np.bool_:
+            raise ValueError("a selection must be a boolean expression")
+        order = _mode.axis_order(binby + [expression])
+        lims = _mode.axis_order(limits)
+        part = taskpart.TaskPartMode(None, shape, order, [float(lim[0]) for lim in lims], [float(lim[1]) for lim in lims], centers,
+                                     selection=mask is not None)
+        task = execution.Task(part, [mask])
+        f.executor.execute(f.columns, [task], f.length, filter=f._filter)
+        return task.result
+
     # ---- binned statistics -------------------------------------------------------------------------------------------
     def _binner_specs(self, binby, limits, shape):
         if binby is None or binby == []:
@@ -527,6 +563,12 @@ class Frame:
 
     def std(self, expression, binby=None, limits=None, shape=128, selection=None, edges=False):
         return self._agg(_agg.std(self._as_float64(expression)), binby, limits, shape, selection, edges)
+
+    def skew(self, expression, binby=None, limits=None, shape=128, selection=None, edges=False):
+        return self._agg(_agg.skew(self._as_float64(expression)), binby, limits, shape, selection, edges)
+
+    def kurtosis(self, expression, binby=None, limits=None, shape=128, selection=None, edges=False):
+        return self._agg(_agg.kurtosis(self._as_float64(expression)), binby, limits, shape, selection, edges)
 
     def min(self, expression, binby=None, limits=None, shape=128, selection=None, edges=False):
         return self._agg(_agg.min(expression), binby, limits, shape, selection, edges)

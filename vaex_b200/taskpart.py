@@ -433,6 +433,57 @@ class TaskPartStatistic(TaskPart):
         return cls(df, **spec)
 
 
+class TaskPartMode(TaskPart):
+    """df.mode (vaex/dataframe.py:2006-2034): vaex.legacy.TaskHistogram's count of binby + [expression] (vaex/legacy.py:22-110) on one
+    device histogram (csrc/statistic.cu, b200_stat_create_histogram), then the argmax finish on that grid; only the modes are read
+    back.  ``expressions`` are in grid axis order, the reference's blocks reversed (mode.axis_order); ``shape``, ``minima`` and
+    ``maxima`` follow them.  Values are binned as float64 (``_asfloat``), masked columns by the values under their mask, as vaexfast
+    reads them; ``selection`` = the task's first selection mask compacts the rows, like a filter does."""
+    snake_name = "mode"
+
+    def __init__(self, df, shape, expressions, minima, maxima, centers, selection=False):
+        from . import mode as _mode
+        self.df = df
+        self.shape = tuple(int(s) for s in shape)
+        self.expressions = list(expressions)
+        self.centers = centers
+        self.selection = bool(selection)
+        self.histogram = _mode.Histogram(self.shape, minima, maxima)
+        self.result = None
+
+    def get_bin_count(self):
+        return reduce(lambda a, b: a * b, self.shape, 1)
+
+    def ideal_splits(self, nthreads):
+        return 1  # one device grid shared by every thread
+
+    def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
+        N = len(blocks[0])
+        columns = []
+        for block in blocks:
+            if _hash.is_string_column(block) or (not _is_device(block) and np.asarray(block).dtype.kind not in "biuf"):
+                raise NotImplementedError("mode of a string, object or datetime column has no GPU path")
+            columns.append(np.ma.getdata(block) if not _is_device(block) and np.ma.isMaskedArray(block) else block)
+        selection = None
+        if self.selection:
+            selection = selection_masks[0]
+            if not _is_device(selection) and np.ma.isMaskedArray(selection):  # unmask_selection_mask
+                selection = np.asarray(selection.data & ~np.ma.getmaskarray(selection))
+        self.histogram.bin(thread_index, columns, [], [selection], N, row_offset=i1)
+        return i2 - i1
+
+    def reduce(self, others):
+        if others:
+            raise ValueError("a mode task part is never split")
+        if self.result is None:
+            self.result = self.histogram.mode(self.centers)
+            self.histogram.close()
+
+    def get_result(self):
+        self.reduce([])
+        return self.result
+
+
 REGISTRY = {cls.snake_name: cls for cls in (TaskPartAggregation, TaskPartHashmapUniqueCreate)}
 
 
