@@ -253,6 +253,32 @@ int b200_set_combine(b200_ctx *ctx, int slot, int nkeys, b200_set *const *sets, 
 int b200_counter_create(b200_ctx *ctx, int dtype, int nmaps, b200_set **out);
 int b200_set_counts(b200_set *set, int64_t *counts_out);
 
+/* ---- index_hash<T>: key -> row number (src/hash_primitives.hpp:731-1040, bound in src/hash_primitives.cpp:57-75; df.join) ---------
+ * A b200_set in index mode: the primary row of a key is its smallest global row (start_index + i), its other rows are its overflow
+ * in ascending order, the NaN / null row is the largest NaN / null row seen.  That is the reference run sequentially, whatever order
+ * the chunks arrive in.  b200_set_destroy applies; every call waits for its work before it returns. */
+int b200_index_create(b200_ctx *ctx, int dtype, int nmaps, b200_set **out); /* index_hash_<T>(nmaps) */
+/* hash_base::_update (:98-295) with index_hash::add_new / add_existing (:776-788); masks: 1 = null */
+int b200_index_update(b200_set *set, int slot, const void *keys, const uint8_t *masks, int64_t nrows, int64_t start_index, int memspace, uint32_t flags);
+/* index_hash::merge (:987-1031): the union of the rows under the rule above */
+int b200_index_merge(b200_set *set, b200_set *const *others, int nothers);
+/* index_hash::map_index_write / map_index_with_mask_write (:793-889): out = nrows rows as int8/16/32/64 (out_isz 1/2/4/8, truncating)
+   in host or device memory; masks may be NULL; *unknown = 1 when a row found nothing */
+int b200_index_map(b200_set *set, int slot, const void *keys, const uint8_t *masks, int64_t nrows, void *out, int out_isz, int32_t *unknown, int memspace,
+                   uint32_t flags);
+/* index_hash::map_index_duplicates (:939-985; the masked form :891-937 is not bound there): *total = the number of
+   (start_index + i, overflow row) pairs; written to left_out / right_out (host or device memory) when total <= capacity.  NaN and
+   masked rows contribute none. */
+int b200_index_duplicates(b200_set *set, int slot, const void *keys, const uint8_t *masks, int64_t nrows, int64_t start_index, int64_t *left_out,
+                          int64_t *right_out, int64_t capacity, int64_t *total, int memspace, uint32_t flags);
+/* the scalar getters (bind_common, src/hash_primitives.cpp:4-25): out[B200_INDEX_INFO_N] */
+enum { B200_INDEX_LENGTH = 0, B200_INDEX_COUNT, B200_INDEX_HAS_DUPLICATES, B200_INDEX_NAN_COUNT, B200_INDEX_NULL_COUNT, B200_INDEX_NAN_ROW,
+       B200_INDEX_NULL_ROW, B200_INDEX_BYTES, B200_INDEX_INFO_N };
+int b200_index_info(b200_set *set, int64_t *out);
+/* hash_base::extract (:330-341): *n_out = the number of distinct keys; when it is at most `capacity`, their canonical 64-bit patterns,
+   primary rows and shards (host memory) */
+int b200_index_extract(b200_set *set, uint64_t *keys_out, int64_t *rows_out, int16_t *shard_out, int64_t capacity, int64_t *n_out);
+
 /* ---- limits pre-pass ------------------------------------------------------------------------ */
 /* out[0] = min, out[1] = max over non-NaN, unmasked values, as double; out = {+inf,-inf} when empty.
  */

@@ -155,6 +155,13 @@ def lib():
             "b200_set_bytes": (sz, [vp]),
             "b200_counter_create": (i32, [vp, i32, i32, P(vp)]),
             "b200_set_counts": (i32, [vp, vp]),
+            "b200_index_create": (i32, [vp, i32, i32, P(vp)]),
+            "b200_index_update": (i32, [vp, i32, vp, vp, i64, i64, i32, u32]),
+            "b200_index_merge": (i32, [vp, P(vp), i32]),
+            "b200_index_map": (i32, [vp, i32, vp, vp, i64, vp, i32, P(C.c_int32), i32, u32]),
+            "b200_index_duplicates": (i32, [vp, i32, vp, vp, i64, i64, vp, vp, i64, P(i64), i32, u32]),
+            "b200_index_info": (i32, [vp, vp]),
+            "b200_index_extract": (i32, [vp, vp, vp, vp, i64, P(i64)]),
             "b200_minmax": (i32, [vp, i32, i32, i32, vp, vp, i64, i32, vp]),
             "b200_stat_create": (i32, [vp, i32, i32, i32, P(i64), P(C.c_double), P(C.c_double), i32, i32, i32, P(vp)]),
             "b200_stat_bin": (i32, [vp, i32, vp, vp, vp, i64, i64, i32, u32]),

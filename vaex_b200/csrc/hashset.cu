@@ -62,16 +62,33 @@ struct b200_set {
     int64_t n_keys = 0, nan_count = 0, null_count = 0;
     int64_t nan_value = 0x7fffffff, null_value = 0x7fffffff; // src/hash_primitives.hpp:447
     int64_t sentinel_ordinal = -1;
+    // index_hash<T> (`indexing`, src/hash_primitives.hpp:731-1040): the table's `first` holds the key's smallest global row (biased,
+    // see index_bias); every non-NaN, non-null row is appended to a row log {canonical key, global row}; the first map_index_duplicates
+    // after a change sorts the log by (table slot, row) into per-slot ranges: primary row first, then the overflow in row order
+    bool indexing = false;
+    b200::DevBuf<unsigned long long> log_key;
+    b200::DevBuf<long long> log_row;
+    uint64_t log_n = 0, log_cap = 0;
+    int64_t row_min = INT64_MAX, row_max = INT64_MIN;
+    bool idx_sorted = false;
+    b200::DevBuf<long long> idx_rows; // the log's rows sorted by (slot, row)
+    b200::DevBuf<uint2> idx_seg;      // per table slot (+1: the key whose pattern is SET_EMPTY): [begin, end) in idx_rows
     std::mutex mu;
 };
 
 namespace b200 {
 
-enum { CTR_COUNT = 0, CTR_OVERFLOW, CTR_NAN_COUNT, CTR_NULL_COUNT, CTR_NAN_TAG, CTR_NULL_TAG, CTR_SENTINEL_TAG, CTR_CURSOR, CTR_SENTINEL_COUNT, CTR_STR_ERROR /* 1: hash == empty pattern, 2: two strings share a 64-bit hash */, CTR_N };
+enum { CTR_COUNT = 0, CTR_OVERFLOW, CTR_NAN_COUNT, CTR_NULL_COUNT, CTR_NAN_TAG, CTR_NULL_TAG, CTR_SENTINEL_TAG, CTR_CURSOR, CTR_SENTINEL_COUNT, CTR_STR_ERROR /* 1: hash == empty pattern, 2: two strings share a 64-bit hash */,
+       CTR_NAN_MAX, CTR_NULL_MAX, CTR_LOG /* index mode: largest biased NaN / null row, rows in the log */, CTR_N };
 
 namespace {
 
 constexpr unsigned long long kTagLowMask = (1ULL << 40) - 1;
+
+// index mode keeps rows as unsigned tags: flipping the sign bit makes unsigned order the signed order of the rows (a negative
+// start_index works), and 0 — the bias of INT64_MIN — stands for "no row" in the NaN / null maxima
+__host__ __device__ __forceinline__ unsigned long long index_bias(long long row) { return (unsigned long long)row ^ (1ull << 63); }
+__host__ __device__ __forceinline__ long long index_unbias(unsigned long long tag) { return (long long)(tag ^ (1ull << 63)); }
 
 __device__ __forceinline__ uint64_t load_raw1(const void *data, int isz, long long i) {
     switch (isz) {
@@ -147,7 +164,7 @@ __global__ void __launch_bounds__(256) k_set_insert(SetSlot *table, unsigned lon
         if ((skip_keys & 1) || dead)
             continue;
         unsigned long long canon = key_canon(dtype, raw);
-        unsigned long long tag = tag_base | (unsigned long long)row;
+        unsigned long long tag = tag_base + (unsigned long long)row; // == tag_base | row for an ordered set (row < 2^40)
         if (canon == SET_EMPTY) {
             atomicMin(ctr + CTR_SENTINEL_TAG, tag);
             continue;
@@ -584,7 +601,7 @@ int64_t set_count_locked(b200_set *s) { return s->n_keys + (s->nan_count > 0) + 
 
 // insert rows [0, nrows) of device arrays; caller holds s->mu
 int set_insert_device(b200_set *s, cudaStream_t st, const void *d_keys, const uint8_t *d_masks, int64_t nrows, bool use_offsets, bool from_keys,
-                      int64_t from_keys_null_index) {
+                      int64_t from_keys_null_index, int64_t start_index = 0) {
     unsigned long long h[CTR_N];
     int skip_keys = 0;
     if (s->limit >= 0) { // hash_primitives.hpp:237-249: a full set skips the whole flush of this call
@@ -592,7 +609,7 @@ int set_insert_device(b200_set *s, cudaStream_t st, const void *d_keys, const ui
         if (set_count_locked(s) >= s->limit)
             skip_keys = 1;
     }
-    const unsigned long long tag_base = from_keys ? 0ull : ((unsigned long long)s->seq << 40);
+    const unsigned long long tag_base = s->indexing ? index_bias(start_index) : from_keys ? 0ull : ((unsigned long long)s->seq << 40);
     s->seq++;
     s->max_call_rows = std::max<int64_t>(s->max_call_rows, nrows);
     const unsigned long long first_low = kTagLowMask - 1, second_low = kTagLowMask;
@@ -636,6 +653,415 @@ int set_insert_device(b200_set *s, cudaStream_t st, const void *d_keys, const ui
     }
     B200_CUDA(cudaGetLastError());
     s->dirty = true;
+    return B200_OK;
+}
+
+// ---- index_hash<T> (src/hash_primitives.hpp:731-1040) ----------------------------------------------------------------------------
+
+// the row log of one update: every non-NaN, non-null row appends {canonical key, global row} (one cursor bump per warp); NaN / null
+// rows raise the largest biased NaN / null row.  Runs once per update, after its insert pass succeeded.
+__global__ void __launch_bounds__(256) k_index_log(unsigned long long *ctr, int dtype, int isz, const void *keys, const uint8_t *masks, long long nrows,
+                                                   long long start, unsigned long long *log_key, long long *log_row) {
+    const unsigned lane = threadIdx.x & 31;
+    unsigned long long nan_max = 0, null_max = 0;
+    for (long long base = (long long)blockIdx.x * blockDim.x; base < nrows; base += (long long)gridDim.x * blockDim.x) {
+        const long long i = base + threadIdx.x; // every lane of a warp runs the same iterations: the ballot below sees all 32
+        bool keep = false;
+        unsigned long long canon = 0;
+        if (i < nrows) {
+            const uint64_t raw = load_raw1(keys, isz, i);
+            if (masks && masks[i])
+                null_max = max(null_max, index_bias(start + i));
+            else if (raw_isnan(dtype, raw))
+                nan_max = max(nan_max, index_bias(start + i));
+            else
+                keep = true, canon = key_canon(dtype, raw);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, keep);
+        unsigned long long pos = 0;
+        if (lane == 0 && m)
+            pos = atomicAdd(ctr + CTR_LOG, (unsigned long long)__popc(m));
+        pos = __shfl_sync(0xffffffffu, pos, 0) + __popc(m & ((1u << lane) - 1u));
+        if (keep) {
+            log_key[pos] = canon;
+            log_row[pos] = start + i;
+        }
+    }
+    if (nan_max)
+        atomicMax(ctr + CTR_NAN_MAX, nan_max);
+    if (null_max)
+        atomicMax(ctr + CTR_NULL_MAX, null_max);
+}
+
+// the slot of a key known to be present (a rehash may have placed it past kMaxProbe: bounded by the empty slot only); the key whose
+// pattern is SET_EMPTY lives outside the table, at slot `cap`
+__device__ __forceinline__ unsigned long long index_slot(const SetSlot *table, unsigned long long mask, unsigned long long canon) {
+    if (canon == SET_EMPTY)
+        return mask + 1;
+    unsigned long long h = hash64(canon) & mask;
+    while (true) {
+        const unsigned long long k = table[h].key;
+        if (k == canon)
+            return h;
+        if (k == SET_EMPTY)
+            return ~0ull;
+        h = (h + 1) & mask;
+    }
+}
+
+// radix input: sort key = row - row_min, payload = slot << 32 (the shard-pass layout of radix.cuh: from_val digits)
+__global__ void k_index_sort_keys(const SetSlot *table, unsigned long long mask, const unsigned long long *log_key, const long long *log_row,
+                                  unsigned long long n, long long row_min, unsigned long long *key, unsigned long long *val) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        key[i] = (unsigned long long)(log_row[i] - row_min);
+        val[i] = index_slot(table, mask, log_key[i]) << 32;
+    }
+}
+
+// sorted by (slot, row): rows back to global rows, and every slot's [begin, end)
+__global__ void k_index_segments(const unsigned long long *key, const unsigned long long *val, unsigned long long n, long long row_min, long long *rows,
+                                 uint2 *seg) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long slot = val[i] >> 32;
+        rows[i] = (long long)key[i] + row_min;
+        if (i == 0 || (val[i - 1] >> 32) != slot)
+            seg[slot].x = (unsigned)i;
+        if (i == n - 1 || (val[i + 1] >> 32) != slot)
+            seg[slot].y = (unsigned)(i + 1);
+    }
+}
+
+// looked-up row of one key: NaN -> the NaN row, masked -> the null row (each -1 and "unknown" when absent), else the primary row
+struct IndexSpecials {
+    long long nan_row, null_row, sent_row; // -1: absent
+    bool sent_present;
+};
+__device__ __forceinline__ IndexSpecials index_specials(const unsigned long long *ctr) {
+    IndexSpecials x;
+    x.nan_row = ctr[CTR_NAN_COUNT] ? index_unbias(ctr[CTR_NAN_MAX]) : -1;
+    x.null_row = ctr[CTR_NULL_COUNT] ? index_unbias(ctr[CTR_NULL_MAX]) : -1;
+    x.sent_present = ctr[CTR_SENTINEL_TAG] != ~0ull;
+    x.sent_row = x.sent_present ? index_unbias(ctr[CTR_SENTINEL_TAG]) : -1;
+    return x;
+}
+
+// index_hash::map_index_write / map_index_with_mask_write (src/hash_primitives.hpp:793-889): out_isz 1/2/4/8 truncates like the
+// reference's assignment into an int8..int64 array
+__global__ void __launch_bounds__(256) k_index_map(const SetSlot *table, unsigned long long mask, const unsigned long long *ctr, int dtype, int isz,
+                                                   const void *keys, const uint8_t *masks, long long nrows, void *out, int out_isz, int *unknown) {
+    const IndexSpecials sp = index_specials(ctr);
+    bool unk = false;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
+        const uint64_t raw = load_raw1(keys, isz, i);
+        long long v;
+        if (raw_isnan(dtype, raw)) {
+            v = sp.nan_row;
+            unk |= v == -1;
+        } else if (masks && masks[i]) {
+            v = sp.null_row;
+            unk |= v == -1;
+        } else {
+            const unsigned long long canon = key_canon(dtype, raw);
+            bool found = false;
+            v = -1;
+            if (canon == SET_EMPTY) {
+                found = sp.sent_present;
+                v = sp.sent_row;
+            } else {
+                unsigned long long h = hash64(canon) & mask;
+                while (true) {
+                    const ulonglong2 s = __ldg(reinterpret_cast<const ulonglong2 *>(table + h));
+                    if (s.x == canon) {
+                        found = true;
+                        v = index_unbias(s.y);
+                        break;
+                    }
+                    if (s.x == SET_EMPTY)
+                        break;
+                    h = (h + 1) & mask;
+                }
+            }
+            unk |= !found;
+        }
+        switch (out_isz) {
+        case 1: static_cast<signed char *>(out)[i] = (signed char)v; break;
+        case 2: static_cast<short *>(out)[i] = (short)v; break;
+        case 4: static_cast<int *>(out)[i] = (int)v; break;
+        default: static_cast<long long *>(out)[i] = v; break;
+        }
+    }
+    if (unk)
+        *unknown = 1;
+}
+
+// the overflow range of a left row's key: [begin + 1, end) of its slot (the primary row is excluded); NaN and masked rows have none
+__device__ __forceinline__ uint2 index_overflow(const SetSlot *table, unsigned long long mask, const uint2 *seg, int dtype, int isz, const void *keys,
+                                                const uint8_t *masks, long long i) {
+    const uint64_t raw = load_raw1(keys, isz, i);
+    if ((masks && masks[i]) || raw_isnan(dtype, raw))
+        return make_uint2(0, 0);
+    const unsigned long long slot = index_slot(table, mask, key_canon(dtype, raw));
+    if (slot == ~0ull)
+        return make_uint2(0, 0);
+    const uint2 r = seg[slot];
+    return r.y > r.x + 1 ? make_uint2(r.x + 1, r.y) : make_uint2(0, 0);
+}
+
+// index_hash::map_index_duplicates (src/hash_primitives.hpp:939-985): pass 1 counts every left row's extra matches (cnt[nrows] = 0,
+// so the exclusive scan leaves the total there) and notes where its range starts in the sorted rows; pass 2 writes the pairs
+// (start + i, overflow row), grouped by left row in left-row order
+__global__ void __launch_bounds__(256) k_index_dup_count(const SetSlot *table, unsigned long long mask, const uint2 *seg, int dtype, int isz, const void *keys,
+                                                         const uint8_t *masks, long long nrows, long long *cnt, unsigned *begin) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= nrows; i += (long long)gridDim.x * blockDim.x) {
+        if (i == nrows) {
+            cnt[i] = 0;
+            continue;
+        }
+        const uint2 r = index_overflow(table, mask, seg, dtype, isz, keys, masks, i);
+        cnt[i] = (long long)(r.y - r.x);
+        begin[i] = r.x;
+    }
+}
+
+// one thread per OUTPUT pair, not per left row: a key with millions of rows would otherwise leave one thread writing them all while
+// the grid idles.  The pair's left row is the last i with off[i] <= o (rows without pairs have off[i] == off[i + 1]).
+__global__ void __launch_bounds__(256) k_index_dup_write(const long long *rows, const long long *off, const unsigned *begin, long long nrows, long long total,
+                                                         long long start, long long *left, long long *right) {
+    for (long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += (long long)gridDim.x * blockDim.x) {
+        long long lo = 0, hi = nrows; // invariant: off[lo] <= o < off[hi]
+        while (hi - lo > 1) {
+            const long long mid = lo + ((hi - lo) >> 1);
+            if (__ldg(off + mid) <= o)
+                lo = mid;
+            else
+                hi = mid;
+        }
+        left[o] = start + lo;
+        right[o] = rows[begin[lo] + (o - off[lo])];
+    }
+}
+
+// merge: every key of the other table enters with its primary row (atomicMin keeps the smaller); on overflow the host grows the
+// table and redoes the pass (idempotent)
+__global__ void __launch_bounds__(256) k_index_merge_table(const SetSlot *other, unsigned long long other_cap, SetSlot *table, unsigned long long mask,
+                                                           unsigned long long *ctr) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < other_cap; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const SetSlot s = other[i];
+        if (s.key == SET_EMPTY)
+            continue;
+        if (!table_insert(table, mask, s.key, s.first)) {
+            ctr[CTR_OVERFLOW] = 1ull;
+            return;
+        }
+    }
+}
+
+// merge: the other index's counters join this one's (its log was appended behind this one's)
+__global__ void k_index_merge_ctr(unsigned long long *ctr, const unsigned long long *other) {
+    atomicAdd(ctr + CTR_NAN_COUNT, other[CTR_NAN_COUNT]);
+    atomicAdd(ctr + CTR_NULL_COUNT, other[CTR_NULL_COUNT]);
+    atomicAdd(ctr + CTR_LOG, other[CTR_LOG]);
+    atomicMin(ctr + CTR_SENTINEL_TAG, other[CTR_SENTINEL_TAG]);
+    atomicMax(ctr + CTR_NAN_MAX, other[CTR_NAN_MAX]);
+    atomicMax(ctr + CTR_NULL_MAX, other[CTR_NULL_MAX]);
+}
+
+// room for `need` log rows; caller holds s->mu
+int index_log_reserve(b200_set *s, cudaStream_t st, uint64_t need) {
+    if (need <= s->log_cap)
+        return B200_OK;
+    const uint64_t cap = std::max<uint64_t>({need, s->log_cap * 2, 1ull << 16});
+    DevBuf<unsigned long long> key;
+    DevBuf<long long> row;
+    B200_CHECK(key.alloc(s->ctx, cap * 8, "index_hash row log", st));
+    B200_CHECK(row.alloc(s->ctx, cap * 8, "index_hash row log", st));
+    if (s->log_n) {
+        B200_CUDA(cudaMemcpyAsync(key, s->log_key, s->log_n * 8, cudaMemcpyDeviceToDevice, st));
+        B200_CUDA(cudaMemcpyAsync(row, s->log_row, s->log_n * 8, cudaMemcpyDeviceToDevice, st));
+    }
+    B200_CUDA(cudaStreamSynchronize(st));
+    key.unbind(), row.unbind();
+    s->log_key = std::move(key), s->log_row = std::move(row);
+    s->log_cap = cap;
+    return B200_OK;
+}
+
+// distinct keys (table + the SET_EMPTY pattern) and the counters, refreshed after a change; caller holds s->mu
+int index_stats(b200_set *s, cudaStream_t st, unsigned long long *h) {
+    if (s->dirty) {
+        unsigned long long zero = 0;
+        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_CURSOR, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
+        k_set_compact<<<nblocks(s->cap), 256, 0, st>>>(s->table, s->cap, s->d_ctr, nullptr, nullptr, nullptr, s->dtype, s->nmaps);
+        B200_CUDA(cudaGetLastError());
+    }
+    B200_CHECK(read_ctr(s, st, h));
+    if (s->dirty) {
+        s->n_keys = (int64_t)(h[CTR_CURSOR] + (h[CTR_SENTINEL_TAG] != ~0ull));
+        s->dirty = false;
+    }
+    s->nan_count = (int64_t)h[CTR_NAN_COUNT];
+    s->null_count = (int64_t)h[CTR_NULL_COUNT];
+    return B200_OK;
+}
+
+// the log sorted by (slot, row) into per-slot ranges, after a change; caller holds s->mu
+int index_sort(b200_set *s, cudaStream_t st) {
+    if (s->idx_sorted)
+        return B200_OK;
+    const unsigned long long E = s->log_n, nslots = s->cap + 1;
+    B200_CHECK(s->idx_seg.alloc(s->ctx, nslots * sizeof(uint2), "index_hash ranges"));
+    B200_CUDA(cudaMemsetAsync(s->idx_seg, 0, nslots * sizeof(uint2), st));
+    B200_CHECK(s->idx_rows.alloc(s->ctx, (E ? E : 1) * 8, "index_hash ranges"));
+    if (E) {
+        const unsigned nblk = radix_blocks(E);
+        const size_t off_hist = 4 * E * 8;
+        DevBuf<char> work;
+        B200_CHECK(work.alloc(s->ctx, off_hist + (size_t)256 * nblk * 4, "index_hash sort", st));
+        unsigned long long *tin = reinterpret_cast<unsigned long long *>(work.get()), *vin = tin + E, *tout = vin + E, *vout = tout + E;
+        unsigned *hist = reinterpret_cast<unsigned *>(work + off_hist);
+        k_index_sort_keys<<<nblocks(E), 256, 0, st>>>(s->table, s->cap - 1, s->log_key, s->log_row, E, s->row_min, tin, vin);
+        B200_CUDA(cudaGetLastError());
+        auto pass = [&](int shift, int from_val) -> int {
+            k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(tin, vin, E, shift, from_val, hist, nblk, radix_tiles(E));
+            k_scan_u32<<<1, 1024, 0, st>>>(hist, 256ull * nblk);
+            k_radix_scatter<<<nblk, kRadixThreads, 0, st>>>(tin, vin, tout, vout, E, shift, from_val, hist, nblk, radix_tiles(E));
+            B200_CUDA(cudaGetLastError());
+            std::swap(tin, tout);
+            std::swap(vin, vout);
+            return B200_OK;
+        };
+        // LSD: the row bytes that vary, then (stable) the slot bytes
+        const unsigned long long row_span = (unsigned long long)(s->row_max - s->row_min);
+        for (int shift = 0; shift < 64 && (row_span >> shift); shift += 8)
+            B200_CHECK(pass(shift, 0));
+        for (int shift = 0; shift < 32 && (s->cap >> shift); shift += 8)
+            B200_CHECK(pass(shift, 1));
+        k_index_segments<<<nblocks(E), 256, 0, st>>>(tin, vin, E, s->row_min, s->idx_rows, s->idx_seg);
+        B200_CUDA(cudaGetLastError());
+        B200_CUDA(cudaStreamSynchronize(st));
+    }
+    s->idx_sorted = true;
+    return B200_OK;
+}
+
+// b200_set_update of an index: the insert pass, then the row log; the frame's inputs are staged
+int index_update(b200_set *s, CallFrame &call, const void *d_keys, const uint8_t *d_masks, int64_t nrows, int64_t start_index) {
+    if (s->log_n + (uint64_t)nrows >= (1ull << 32)) {
+        set_error("b200_index_update: an index_hash holds at most 2^32 rows");
+        return B200_ERR_UNSUPPORTED;
+    }
+    if (!nrows)
+        return B200_OK;
+    cudaStream_t st = call.st;
+    B200_CHECK(index_log_reserve(s, st, s->log_n + (uint64_t)nrows));
+    B200_CHECK(set_insert_device(s, st, d_keys, d_masks, nrows, true, false, -1, start_index));
+    k_index_log<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->d_ctr, s->dtype, dtype_size(s->dtype), d_keys, d_masks, nrows, start_index, s->log_key,
+                                                                    s->log_row);
+    B200_CUDA(cudaGetLastError());
+    unsigned long long h[CTR_N];
+    B200_CHECK(read_ctr(s, st, h));
+    s->log_n = h[CTR_LOG];
+    s->row_min = std::min<int64_t>(s->row_min, start_index);
+    s->row_max = std::max<int64_t>(s->row_max, start_index + nrows - 1);
+    s->idx_sorted = false;
+    return B200_OK;
+}
+
+// b200_set_merge of one other index, under the sequential rule: the union of both indexes' rows, primary = the smallest row, NaN /
+// null row = the largest; caller holds both locks
+int index_merge_one(b200_set *s, b200_set *o, cudaStream_t st) {
+    if (s->log_n + o->log_n >= (1ull << 32)) {
+        set_error("b200_index_merge: an index_hash holds at most 2^32 rows");
+        return B200_ERR_UNSUPPORTED;
+    }
+    unsigned long long h[CTR_N], ho[CTR_N];
+    B200_CHECK(index_stats(s, st, h));
+    B200_CHECK(index_stats(o, st, ho));
+    uint64_t want = s->cap;
+    while (want < 2 * (uint64_t)(s->n_keys + o->n_keys))
+        want <<= 1;
+    if (want > s->cap)
+        B200_CHECK(set_grow(s, st, want));
+    while (true) {
+        k_index_merge_table<<<nblocks(o->cap), 256, 0, st>>>(o->table, o->cap, s->table, s->cap - 1, s->d_ctr);
+        B200_CUDA(cudaGetLastError());
+        B200_CHECK(read_ctr(s, st, h));
+        if (!h[CTR_OVERFLOW])
+            break;
+        unsigned long long zero = 0;
+        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_OVERFLOW, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
+        B200_CHECK(set_grow(s, st));
+    }
+    B200_CHECK(index_log_reserve(s, st, s->log_n + o->log_n));
+    if (o->log_n) {
+        B200_CUDA(cudaMemcpyAsync(s->log_key + s->log_n, o->log_key, o->log_n * 8, cudaMemcpyDeviceToDevice, st));
+        B200_CUDA(cudaMemcpyAsync(s->log_row + s->log_n, o->log_row, o->log_n * 8, cudaMemcpyDeviceToDevice, st));
+    }
+    k_index_merge_ctr<<<1, 1, 0, st>>>(s->d_ctr, o->d_ctr);
+    B200_CUDA(cudaGetLastError());
+    B200_CHECK(read_ctr(s, st, h));
+    s->log_n = h[CTR_LOG];
+    s->row_min = std::min(s->row_min, o->row_min);
+    s->row_max = std::max(s->row_max, o->row_max);
+    s->dirty = true;
+    s->idx_sorted = false;
+    return B200_OK;
+}
+
+// what set_map_common does for an index: map_index (out = rows of out_isz bytes, *unknown) or map_index_duplicates (out = the left
+// rows, right = the right rows, written when *total <= capacity)
+struct IndexLookup {
+    const uint8_t *masks;
+    int32_t *unknown;
+    bool duplicates;
+    int64_t start;
+    int64_t *right;
+    int64_t capacity;
+    int64_t *total;
+};
+
+// caller holds s->mu; the frame's result rule applies (the entry point finishes it, waiting: the table may grow once the lock is
+// released)
+int index_lookup(b200_set *s, CallFrame &call, const void *keys, int64_t nrows, void *out, int out_isz, const IndexLookup &ix) {
+    cudaStream_t st = call.st;
+    const int isz = dtype_size(s->dtype);
+    call.plan(keys, (size_t)nrows * isz);
+    if (ix.masks)
+        call.plan(ix.masks, (size_t)nrows);
+    B200_CHECK(call.commit());
+    const void *d_keys = call.dev(keys);
+    const uint8_t *d_masks = ix.masks ? static_cast<const uint8_t *>(call.dev(ix.masks)) : nullptr;
+    if (!ix.duplicates) {
+        void *d_out;
+        int *d_unknown;
+        B200_CHECK(call.out(out, (size_t)nrows * out_isz, call.result_on_device(out), &d_out));
+        B200_CHECK(call.out(ix.unknown, sizeof(int32_t), false, &d_unknown));
+        B200_CUDA(cudaMemsetAsync(d_unknown, 0, sizeof(int32_t), st));
+        k_index_map<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->table, s->cap - 1, s->d_ctr, s->dtype, isz, d_keys, d_masks, nrows, d_out, out_isz,
+                                                                       d_unknown);
+        B200_CUDA(cudaGetLastError());
+        return B200_OK;
+    }
+    B200_CHECK(index_sort(s, st));
+    const unsigned long long n1 = (unsigned long long)nrows + 1;
+    const unsigned long long n_off = n1 + scan_i64_sums(n1);
+    DevBuf<long long> off;
+    B200_CHECK(off.alloc(s->ctx, n_off * 8 + (size_t)nrows * 4, "b200_index_duplicates", st));
+    unsigned *begin = reinterpret_cast<unsigned *>(off + n_off);
+    k_index_dup_count<<<nblocks(n1), 256, 0, st>>>(s->table, s->cap - 1, s->idx_seg, s->dtype, isz, d_keys, d_masks, nrows, off, begin);
+    B200_CUDA(cudaGetLastError());
+    B200_CHECK(scan_i64(off, n1, off + n1, st));
+    long long n_out = 0;
+    B200_CUDA(cudaMemcpyAsync(&n_out, off + nrows, 8, cudaMemcpyDeviceToHost, st));
+    B200_CUDA(cudaStreamSynchronize(st));
+    *ix.total = n_out;
+    if (n_out && n_out <= ix.capacity) {
+        long long *d_left, *d_right;
+        B200_CHECK(call.out(out, (size_t)n_out * 8, call.result_on_device(out), &d_left));
+        B200_CHECK(call.out(ix.right, (size_t)n_out * 8, call.result_on_device(ix.right), &d_right));
+        k_index_dup_write<<<nblocks((unsigned long long)n_out), 256, 0, st>>>(s->idx_rows, off, begin, nrows, n_out, ix.start, d_left, d_right);
+        B200_CUDA(cudaGetLastError());
+    }
     return B200_OK;
 }
 
@@ -742,6 +1168,10 @@ int b200_set_update(b200_set *s, int slot, const void *keys, const uint8_t *mask
         set_error("Cannot combine limit with return_inverse"); // hash_primitives.hpp:102-104
         return B200_ERR_STATE;
     }
+    if (s->indexing && return_values) {
+        set_error("b200_set_update: an index_hash returns no values");
+        return B200_ERR_INVALID;
+    }
     if (nrows >= (1ll << 40) - 2) {
         set_error("b200_set_update: more than 2^40 rows in one call");
         return B200_ERR_UNSUPPORTED;
@@ -757,6 +1187,10 @@ int b200_set_update(b200_set *s, int slot, const void *keys, const uint8_t *mask
     B200_CHECK(call.commit());
     const void *d_keys = call.dev(keys);
     const uint8_t *d_masks = masks ? static_cast<const uint8_t *>(call.dev(masks)) : nullptr;
+    if (s->indexing) {
+        B200_CHECK(index_update(s, call, d_keys, d_masks, nrows, start_index));
+        return call.finish(true); // the table may grow once the lock is released
+    }
     const bool use_offsets = return_values || start_index != -1;
     B200_CHECK(set_insert_device(s, st, d_keys, d_masks, nrows, use_offsets, false, -1));
     if (return_values && nrows) {
@@ -829,14 +1263,27 @@ int b200_set_merge(b200_set *s, b200_set *const *others, int nothers) {
         set_error("b200_set_merge: null set");
         return B200_ERR_INVALID;
     }
-    for (int i = 0; i < nothers; i++)
+    for (int i = 0; i < nothers; i++) {
+        if (others[i]->indexing != s->indexing || (s->indexing && (others[i] == s || others[i]->ctx->device != s->ctx->device))) {
+            set_error("b200_set_merge: invalid argument");
+            return B200_ERR_INVALID;
+        }
         if (others[i]->nmaps != s->nmaps || others[i]->dtype != s->dtype) {
             set_error("cannot merge with an unequal maps");
             return B200_ERR_STATE;
         }
+    }
     B200_CUDA(cudaSetDevice(s->ctx->device));
     for (int i = 0; i < nothers; i++) {
         b200_set *o = others[i];
+        if (s->indexing) {
+            CallFrame call(s->ctx, 0, B200_MEM_HOST, 0, "b200_set_merge");
+            B200_CHECK(call.rc);
+            std::scoped_lock g(s->mu, o->mu);
+            B200_CHECK(index_merge_one(s, o, call.st));
+            B200_CHECK(call.finish(true));
+            continue;
+        }
         std::vector<uint64_t> keys, weights;
         std::vector<int64_t> o_counts;
         int64_t o_nan, o_null;
@@ -971,8 +1418,10 @@ int b200_set_ordinal_dtype(b200_set *s) {
 }
 
 // out: nrows results of out_isz bytes (0: isin's one byte) in host or device memory (CallFrame::result_on_device)
-static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows, void *out, int out_isz, int memspace, uint32_t flags, const char *name) {
-    if (!s || nrows < 0) {
+// ix: an index_hash lookup (index_lookup)
+static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows, void *out, int out_isz, int memspace, uint32_t flags, const char *name,
+                          const IndexLookup *ix = nullptr) {
+    if (!s || nrows < 0 || s->indexing != (ix != nullptr)) {
         set_error("%s: invalid argument", name);
         return B200_ERR_INVALID;
     }
@@ -981,6 +1430,10 @@ static int set_map_common(b200_set *s, int slot, const void *keys, int64_t nrows
     if (!nrows)
         return B200_OK;
     std::lock_guard<std::mutex> g(s->mu);
+    if (ix) {
+        B200_CHECK(index_lookup(s, call, keys, nrows, out, out_isz, *ix));
+        return call.finish(true); // the table may grow once the lock is released
+    }
     B200_CHECK(set_finalize(s));
     const size_t isz = dtype_size(s->dtype);
     const size_t osz = out_isz ? out_isz : 1;
@@ -1059,6 +1512,127 @@ size_t b200_set_bytes(b200_set *s) {
     if (set_finalize(s))
         return 0;
     return (size_t)s->n_keys * (dtype_size(s->dtype) + 8);
+}
+
+// ---- index_hash<T> ----------------------------------------------------------------------------------------------------------------
+
+// index_hash_<T>(nmaps) (src/hash_primitives.cpp:57-75)
+int b200_index_create(b200_ctx *ctx, int dtype, int nmaps, b200_set **out) {
+    b200_set *s = nullptr;
+    B200_CHECK(set_create(ctx, dtype, nmaps, -1, false, false, &s));
+    s->indexing = true;
+    *out = s;
+    return B200_OK;
+}
+
+static bool index_check(const b200_set *s, const char *name) {
+    if (!s || !s->indexing || s->strings) {
+        set_error("%s: not an index_hash", name);
+        return false;
+    }
+    return true;
+}
+
+// hash_base::_update (src/hash_primitives.hpp:98-295) with index_hash::add_new / add_existing (:776-788), through b200_set_update
+int b200_index_update(b200_set *s, int slot, const void *keys, const uint8_t *masks, int64_t nrows, int64_t start_index, int memspace, uint32_t flags) {
+    if (!index_check(s, "b200_index_update"))
+        return B200_ERR_INVALID;
+    return b200_set_update(s, slot, keys, masks, nrows, start_index, 0, nullptr, nullptr, memspace, flags);
+}
+
+// index_hash::merge (src/hash_primitives.hpp:987-1031), through b200_set_merge
+int b200_index_merge(b200_set *s, b200_set *const *others, int nothers) {
+    if (!index_check(s, "b200_index_merge"))
+        return B200_ERR_INVALID;
+    return b200_set_merge(s, others, nothers);
+}
+
+// index_hash::map_index_write / map_index_with_mask_write (src/hash_primitives.hpp:793-889)
+int b200_index_map(b200_set *s, int slot, const void *keys, const uint8_t *masks, int64_t nrows, void *out, int out_isz, int32_t *unknown, int memspace,
+                   uint32_t flags) {
+    if (!index_check(s, "b200_index_map"))
+        return B200_ERR_INVALID;
+    if (nrows < 0 || (nrows && (!keys || !out)) || !unknown || (out_isz != 1 && out_isz != 2 && out_isz != 4 && out_isz != 8)) {
+        set_error("b200_index_map: invalid argument");
+        return B200_ERR_INVALID;
+    }
+    *unknown = 0;
+    IndexLookup ix{masks, unknown, false, 0, nullptr, 0, nullptr};
+    return set_map_common(s, slot, keys, nrows, out, out_isz, memspace, flags, "b200_index_map", &ix);
+}
+
+// index_hash::map_index_duplicates (src/hash_primitives.hpp:939-985; the masked form :891-937 is not bound)
+int b200_index_duplicates(b200_set *s, int slot, const void *keys, const uint8_t *masks, int64_t nrows, int64_t start_index, int64_t *left_out,
+                          int64_t *right_out, int64_t capacity, int64_t *total, int memspace, uint32_t flags) {
+    if (!index_check(s, "b200_index_duplicates"))
+        return B200_ERR_INVALID;
+    if (nrows < 0 || (nrows && !keys) || !total || capacity < 0 || (capacity && (!left_out || !right_out))) {
+        set_error("b200_index_duplicates: invalid argument");
+        return B200_ERR_INVALID;
+    }
+    *total = 0;
+    IndexLookup ix{masks, nullptr, true, start_index, right_out, capacity, total};
+    return set_map_common(s, slot, keys, nrows, left_out, 8, memspace, flags, "b200_index_duplicates", &ix);
+}
+
+// out[B200_INDEX_INFO_N]: the scalar getters (bind_common, src/hash_primitives.cpp:4-25, and index_hash :750-759, :1037)
+int b200_index_info(b200_set *s, int64_t *out) {
+    if (!index_check(s, "b200_index_info") || !out)
+        return B200_ERR_INVALID;
+    B200_CUDA(cudaSetDevice(s->ctx->device));
+    std::lock_guard<std::mutex> g(s->mu);
+    unsigned long long h[CTR_N];
+    B200_CHECK(index_stats(s, s->ctx->slots[0]->stream, h));
+    const int64_t specials = (s->nan_count > 0) + (s->null_count > 0);
+    out[B200_INDEX_LENGTH] = (int64_t)s->log_n + specials;
+    out[B200_INDEX_COUNT] = s->n_keys + specials;
+    out[B200_INDEX_HAS_DUPLICATES] = (int64_t)s->log_n > s->n_keys;
+    out[B200_INDEX_NAN_COUNT] = s->nan_count;
+    out[B200_INDEX_NULL_COUNT] = s->null_count;
+    out[B200_INDEX_NAN_ROW] = s->nan_count ? index_unbias(h[CTR_NAN_MAX]) : -1;
+    out[B200_INDEX_NULL_ROW] = s->null_count ? index_unbias(h[CTR_NULL_MAX]) : -1;
+    out[B200_INDEX_BYTES] = (int64_t)(s->cap * sizeof(SetSlot) + s->log_cap * 16);
+    return B200_OK;
+}
+
+// hash_base::extract (src/hash_primitives.hpp:330-341): every distinct key (canonical pattern, host), its primary row and its shard;
+// *n_out = their number, written to the arrays when it is at most `capacity`
+int b200_index_extract(b200_set *s, uint64_t *keys_out, int64_t *rows_out, int16_t *shard_out, int64_t capacity, int64_t *n_out) {
+    if (!index_check(s, "b200_index_extract") || !n_out || capacity < 0 || (capacity && (!keys_out || !rows_out || !shard_out)))
+        return B200_ERR_INVALID;
+    B200_CUDA(cudaSetDevice(s->ctx->device));
+    std::lock_guard<std::mutex> g(s->mu);
+    cudaStream_t st = s->ctx->slots[0]->stream;
+    unsigned long long h[CTR_N];
+    B200_CHECK(index_stats(s, st, h));
+    const bool has_sent = h[CTR_SENTINEL_TAG] != ~0ull;
+    const uint64_t n = (uint64_t)s->n_keys - has_sent;
+    *n_out = s->n_keys;
+    if ((uint64_t)s->n_keys > (uint64_t)capacity)
+        return B200_OK;
+    if (n) {
+        DevBuf<unsigned long long> work;
+        B200_CHECK(work.alloc(s->ctx, n * 24, "b200_index_extract", st));
+        unsigned long long zero = 0;
+        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_CURSOR, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
+        k_set_compact<<<nblocks(s->cap), 256, 0, st>>>(s->table, s->cap, s->d_ctr, work, work + n, work + 2 * n, s->dtype, s->nmaps);
+        B200_CUDA(cudaGetLastError());
+        std::vector<unsigned long long> v(n);
+        B200_CUDA(cudaMemcpyAsync(keys_out, work, n * 8, cudaMemcpyDeviceToHost, st));
+        B200_CUDA(cudaMemcpyAsync(rows_out, work + n, n * 8, cudaMemcpyDeviceToHost, st));
+        B200_CUDA(cudaMemcpyAsync(v.data(), work + 2 * n, n * 8, cudaMemcpyDeviceToHost, st));
+        B200_CUDA(cudaStreamSynchronize(st));
+        for (uint64_t i = 0; i < n; i++) {
+            rows_out[i] = index_unbias((unsigned long long)rows_out[i]);
+            shard_out[i] = (int16_t)(v[i] >> 32);
+        }
+    }
+    if (has_sent) {
+        keys_out[n] = SET_EMPTY;
+        rows_out[n] = index_unbias(h[CTR_SENTINEL_TAG]);
+        shard_out[n] = (int16_t)(key_hash(s->dtype, SET_EMPTY) % (unsigned long long)s->nmaps);
+    }
+    return B200_OK;
 }
 
 uint64_t b200_hash64(uint64_t x) { return hash64(x); }

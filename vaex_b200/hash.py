@@ -30,6 +30,20 @@ def ordered_set_type_from_dtype(dtype):
     return getattr(superutils, name)
 
 
+def index_type_from_dtype(dtype, transient=True, prime_growth=False):
+    """vaex.hash.index_type_from_dtype (vaex/hash.py:56-60, vaex/utils.py:754-790 with support_non_native=False): the index_hash
+    class for a key dtype; datetimes and timedeltas are indexed as int64, and a byte-swapped dtype has no class (big-endian float64
+    excepted, which the reference maps to float64).  ``transient`` and ``prime_growth`` only choose the CPU table's string storage
+    and growth policy, so they change nothing here.  String keys have no device index yet."""
+    if str(dtype) == "string" or np.dtype(dtype).kind in "OUS":
+        raise TypeError(f"no index_hash for dtype {dtype}: string keys are not indexed on the device")
+    dtype = np.dtype(dtype)
+    name = "float64" if str(dtype) == ">f8" else "int64" if dtype.kind in "mM" else str(dtype)
+    if not hasattr(superutils, "index_hash_" + name):
+        raise ValueError(f"Could not find a class (index_hash_{name}), seems {dtype} is not supported.")
+    return getattr(superutils, "index_hash_" + name)
+
+
 class HashMapUnique:
     """HashMap that maps keys to unique integers (vaex/hash.py:62-64)."""
 

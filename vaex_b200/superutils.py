@@ -297,6 +297,196 @@ for _name in _lib.DTYPES:
     globals()["counter_" + _name] = _cls
 
 
+_INDEX_OUT = {np.dtype(t): np.dtype(t).itemsize for t in ("int8", "int16", "int32", "int64")}
+
+
+class _IndexHash:
+    """``vaex.superutils.index_hash_<dtype>(nmaps)`` (src/hash_primitives.hpp:731-1040, bound in src/hash_primitives.cpp:57-75):
+    key -> row number, what ``df.join`` runs on.  A key's primary row is its smallest row (``start_index + i``) and its other rows
+    are its overflow, in ascending order; the NaN / null row is the largest NaN / null row seen.  That is the reference run
+    sequentially, one ``update`` per chunk in order, whatever order the chunks arrive in; where the reference's own answer depends
+    on chunk order (merges, NaN / null rows of later calls), DESIGN.md states the difference."""
+    _dtype = None
+    _code = None
+    _key_column = _OrderedSet._key_column
+    __del__ = _OrderedSet.__del__
+
+    @classmethod
+    def _np_dtype(cls):
+        return np.dtype(cls._dtype)
+
+    def __init__(self, nmaps=1):
+        self._ctx = _lib.context()
+        self._h = C.c_void_p()
+        self.sealed = False
+        self.nmaps = int(nmaps)
+        _lib.check(_lib.lib().b200_index_create(self._ctx._h, self._code, self.nmaps, C.byref(self._h)))
+
+    def _lookup_column(self, values):
+        """map_index takes ``py::array_t<T>`` without forcecast: numpy converts only where the cast is safe (int32 keys on an int64
+        index), anything else is a TypeError.  Device columns follow ``_key_column``."""
+        native = self._np_dtype()
+        if isinstance(values, np.ndarray) and not np.can_cast(values.dtype, native, "safe"):
+            raise TypeError(f"{type(self).__name__}.map_index: incompatible key dtype {values.dtype} (index dtype {native})")
+        if not isinstance(values, np.ndarray) and getattr(values, "__cuda_array_interface__", None) is None:
+            values = np.asarray(values, dtype=native)
+        return self._key_column(values)
+
+    def _info(self):
+        out = np.zeros(8, np.int64)
+        _lib.check(_lib.lib().b200_index_info(self._h, out.ctypes.data))
+        return out
+
+    # -- reference protocol --------------------------------------------------------------------------
+    def update(self, values, *args, **kwargs):
+        """update(values[, masks], start_index=0, chunk_size=..., bucket_size=..., return_values=False)"""
+        names = ["start_index", "chunk_size", "bucket_size", "return_values"]
+        masks = kwargs.pop("masks", None)
+        args = list(args)
+        if args and not isinstance(args[0], (int, np.integer, bool)):
+            masks = args.pop(0)
+        opts = dict(start_index=0, chunk_size=1024 * 128, bucket_size=1024 * 128, return_values=False)
+        opts.update(zip(names, args))
+        opts.update(kwargs)
+        if opts["bucket_size"] < opts["chunk_size"]:
+            raise RuntimeError("bucket size should be larger than chunk_size")
+        if opts["return_values"]:
+            raise RuntimeError("index_hash: return_values is not supported")
+        if self.sealed:
+            raise RuntimeError("hashmap is sealed, cannot update")
+        col = self._key_column(values)
+        mcol = None
+        if masks is not None:
+            mcol = _lib.mask_column(masks)
+            if mcol.length != col.length:
+                raise RuntimeError("array and mask should be of same size")
+        _lib.check(_lib.lib().b200_index_update(self._h, 0, col.ptr, None if mcol is None else mcol.ptr, col.length, int(opts["start_index"]),
+                                                _lib.memspace(col, mcol), 0))
+
+    def merge(self, other):
+        if self.sealed:
+            raise RuntimeError("hashmap is sealed, cannot merge")
+        others = other if isinstance(other, (list, tuple)) else [other]
+        arr = (C.c_void_p * len(others))(*[o._h for o in others])
+        _lib.check(_lib.lib().b200_index_merge(self._h, arr, len(others)))
+
+    def _map(self, values, mask, out):
+        col = self._lookup_column(values)
+        mcol = None if mask is None else _lib.mask_column(mask)
+        if mcol is not None and mcol.length != col.length:
+            raise RuntimeError("array and mask should be of same size")
+        give = out is None
+        if give:
+            if col.memspace == _lib.MEM_DEVICE:
+                import torch
+                out = torch.empty(col.length, dtype=torch.int64, device=f"cuda:{self._ctx.device}")
+            else:
+                out = np.empty(col.length, np.int64)
+        ocol = _lib.column(out)
+        if ocol.dtype not in _INDEX_OUT or ocol.length < col.length:
+            raise TypeError(f"map_index: out must be an int8, int16, int32 or int64 array of at least {col.length} rows")
+        unknown = C.c_int32(0)
+        if col.length:
+            _lib.check(_lib.lib().b200_index_map(self._h, 0, col.ptr, None if mcol is None else mcol.ptr, col.length, ocol.ptr, _INDEX_OUT[ocol.dtype],
+                                                 C.byref(unknown), _lib.memspace(col, mcol, ocol), 0))
+        if isinstance(out, np.ndarray) and ocol.keep is not out:
+            out[:] = ocol.keep  # a non-contiguous host `out` was written through a copy
+        return out if give else bool(unknown.value)
+
+    def map_index(self, values, out=None):
+        """map_index(values) -> int64 rows (-1: not found); map_index(values, out) writes int8..int64 ``out`` (truncating) and returns
+        whether a key was not found"""
+        return self._map(values, None, out)
+
+    def map_index_masked(self, values, mask, out=None):
+        return self._map(values, mask, out)
+
+    def map_index_duplicates(self, values, start_index, mask=None, device=False):
+        """(left rows, right rows): for every row i of `values` whose key has an overflow, ``start_index + i`` paired with each overflow
+        row.  `mask` (masked rows contribute none) and `device` (torch results on the index's GPU) are this project's additions."""
+        col = self._lookup_column(values)
+        mcol = None if mask is None else _lib.mask_column(mask)
+        lib, ms = _lib.lib(), _lib.memspace(col, mcol)
+        total = C.c_int64(0)
+        args = (self._h, 0, col.ptr, None if mcol is None else mcol.ptr, col.length, int(start_index))
+        _lib.check(lib.b200_index_duplicates(*args, None, None, 0, C.byref(total), ms, 0))
+        while True:  # the pairs are written only when they fit: an update from another thread in between changes the total
+            n = total.value
+            if device:
+                import torch
+                left, right = (torch.empty(n, dtype=torch.int64, device=f"cuda:{self._ctx.device}") for _ in range(2))
+                lp, rp = left.data_ptr(), right.data_ptr()
+            else:
+                left, right = np.empty(n, np.int64), np.empty(n, np.int64)
+                lp, rp = left.ctypes.data, right.ctypes.data
+            if not n:
+                break
+            _lib.check(lib.b200_index_duplicates(*args, lp, rp, n, C.byref(total), _lib.memspace(col, mcol, _lib.column(left)), 0))
+            if total.value == n:
+                break
+        return left, right
+
+    has_duplicates = property(lambda self: bool(self._info()[2]))
+    nan_count = property(lambda self: int(self._info()[3]))
+    null_count = property(lambda self: int(self._info()[4]))
+    has_nan = property(lambda self: self.nan_count > 0)
+    has_null = property(lambda self: self.null_count > 0)
+    count = property(lambda self: int(self._info()[1]))
+
+    def __len__(self):
+        return int(self._info()[0])
+
+    def _nan_row(self):
+        return int(self._info()[5])
+
+    def _null_row(self):
+        return int(self._info()[6])
+
+    def seal(self):
+        self.sealed = True
+
+    def _extract_arrays(self):
+        n = C.c_int64(0)
+        _lib.check(_lib.lib().b200_index_extract(self._h, None, None, None, 0, C.byref(n)))
+        while True:  # written only when it fits: an update from another thread in between changes the count
+            cap = n.value
+            keys, rows, shards = np.empty(cap, np.uint64), np.empty(cap, np.int64), np.empty(cap, np.int16)
+            _lib.check(_lib.lib().b200_index_extract(self._h, keys.ctypes.data, rows.ctypes.data, shards.ctypes.data, cap, C.byref(n)))
+            if n.value <= cap:
+                keys, rows, shards = keys[:n.value], rows[:n.value], shards[:n.value]
+                break
+        native = self._np_dtype()
+        keys = keys.astype(np.dtype(f"u{native.itemsize}")).view(native)  # canonical patterns -> the key's own bits
+        return keys, rows, shards
+
+    def extract(self):
+        keys, rows, shards = self._extract_arrays()
+        maps = [{} for _ in range(self.nmaps)]
+        for k, r, m in zip(keys.tolist(), rows.tolist(), shards.tolist()):
+            maps[m][k] = r
+        return maps
+
+    def offsets(self):
+        # hash_common::offsets (src/hash.hpp:337-353): shard 0 also holds the NaN / null entries
+        _, _, shards = self._extract_arrays()
+        sizes = np.bincount(shards, minlength=self.nmaps).astype(np.int64)
+        sizes[0] += self.offset
+        return [0] + np.cumsum(sizes)[:-1].tolist()
+
+    @property
+    def offset(self):
+        return int(self.null_count > 0) + int(self.nan_count > 0)
+
+    def __sizeof__(self):
+        return int(self._info()[7])
+
+
+for _name in _lib.DTYPES:
+    _cls = type("index_hash_" + _name, (_IndexHash,), dict(_dtype=_name, _code=_lib.DTYPE_CODE[_name]))
+    _cls.__module__ = __name__
+    globals()["index_hash_" + _name] = _cls
+
+
 # ---- string keys (src/hash_string.hpp, bound in src/hash_string.cpp:86-99 as ordered_set_string) ------------------------------------
 def string_buffers(values):
     """strings -> (int64 offsets[n + 1], uint8 bytes, uint8 null mask or None): the arrow large_string layout the reference's
