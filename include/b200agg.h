@@ -397,6 +397,25 @@ int b200_eval(b200_ctx *ctx, int slot, const b200_expr_op *prog, int nops, const
 int b200_compact(b200_ctx *ctx, int slot, const uint8_t *keep, int ncols, const void *const *cols, const int32_t *dtypes, int64_t nrows, int memspace,
                  void *const *outs_device, int64_t *count_out);
 
+/* ---- take: the row gather of df.join (vaex/join.py:286 right_dataset.take(lookup, masked=...), :214 left.take(lookup_left), :218-222
+ * the inner join's matched rows) ----------------------------------------------------------------------------------------------
+ * index: n rows of int8/16/32/64 (index_isz 1/2/4/8), the row of the source each output row takes; < 0 = missing (value 0, validity
+ * 0); >= src_len fails with B200_ERR_INVALID (the reference fills its lookup with iinfo.max so that such a bug crashes, :178-181).
+ * Up to 16 columns of src_len items of 1/2/4/8 bytes; src_masks (may be NULL, or NULL per column): 1 = missing, which stays missing.
+ * dst[c] receives n items, dst_valid (may be NULL, or NULL per column) n bytes, 1 = valid.  Every pointer is device memory: a join
+ * stages a host column once, not once per call.  missing_out[c] (host) = 1 when column c has a missing output row (:286
+ * `masked=any(lookup_masked)`).  Runs on the slot's stream and waits for its work. */
+int b200_take(b200_ctx *ctx, int slot, const void *index, int index_isz, int64_t n, int ncols, const void *const *src, const int32_t *src_isz,
+              const uint8_t *const *src_masks, int64_t src_len, void *const *dst, uint8_t *const *dst_valid, int32_t *missing_out);
+/* the same gather for an arrow string column: offsets = src_len + 1 int32 or int64 values (offset_isz 4/8, a sliced array's own
+ * offsets), bytes = the buffer those offsets index, src_mask (may be NULL): 1 = missing.  Output: the large_string layout, offsets_out
+ * = n + 1 int64 from 0, valid_out (may be NULL) n bytes, 1 = valid; a missing row is an empty null string.  *size_needed = the output's
+ * byte count; the bytes are written to bytes_out only when it fits in `capacity` (b200_index_extract's protocol: offsets_out,
+ * valid_out and *missing_out are written on every call).  Inputs and outputs are device memory, size_needed and missing_out host. */
+int b200_take_strings(b200_ctx *ctx, int slot, const void *index, int index_isz, int64_t n, const void *offsets, int offset_isz, const uint8_t *bytes,
+                      const uint8_t *src_mask, int64_t src_len, int64_t *offsets_out, uint8_t *bytes_out, uint8_t *valid_out, int64_t capacity,
+                      int64_t *size_needed, int32_t *missing_out);
+
 
 /* ---- host-chunk ingestion (SURVEY.md 8f row 2) ---------------------------------------------- */
 /* Page-lock a host column once (cudaHostRegister) so that the per-chunk H2D copies of b200_bin(HOST) run at PCIe rate and

@@ -153,42 +153,6 @@ __global__ void k_list_str_len(const unsigned long long *vals, const unsigned lo
     }
 }
 
-// 16 bytes of the byte stream that starts `mis` (1..15) bytes into the aligned word `a`, followed by `b`
-__device__ __forceinline__ uint4 shift16(uint4 a, uint4 b, int mis) {
-    const int q = mis >> 2;
-    const unsigned r = (unsigned)(mis & 3) * 8;
-    const unsigned w0 = q == 0 ? a.x : q == 1 ? a.y : q == 2 ? a.z : a.w;
-    const unsigned w1 = q == 0 ? a.y : q == 1 ? a.z : q == 2 ? a.w : b.x;
-    const unsigned w2 = q == 0 ? a.z : q == 1 ? a.w : q == 2 ? b.x : b.y;
-    const unsigned w3 = q == 0 ? a.w : q == 1 ? b.x : q == 2 ? b.y : b.z;
-    const unsigned w4 = q == 0 ? b.x : q == 1 ? b.y : q == 2 ? b.z : b.w;
-    return make_uint4(__funnelshift_r(w0, w1, r), __funnelshift_r(w1, w2, r), __funnelshift_r(w2, w3, r), __funnelshift_r(w3, w4, r));
-}
-
-// G threads copy one string: single bytes up to the first 16-byte boundary of the destination, then 16-byte stores (16-byte loads
-// when source and destination are equally misaligned, else two aligned loads and a funnel shift), then the last bytes.  The source
-// reads may run up to 16 bytes past the string: the pool is allocated with that much slack.
-template <int G>
-__device__ __forceinline__ void copy_string(char *dst, const char *src, long long len, int lane) {
-    const long long head = min(len, (long long)((16 - (reinterpret_cast<uintptr_t>(dst) & 15)) & 15));
-    for (long long c = lane; c < head; c += G)
-        dst[c] = src[c];
-    const long long chunks = (len - head) >> 4;
-    uint4 *d = reinterpret_cast<uint4 *>(dst + head);
-    const char *s = src + head;
-    const int mis = (int)(reinterpret_cast<uintptr_t>(s) & 15);
-    const uint4 *s4 = reinterpret_cast<const uint4 *>(s - mis);
-    if (mis == 0) {
-        for (long long c = lane; c < chunks; c += G)
-            d[c] = __ldg(s4 + c);
-    } else {
-        for (long long c = lane; c < chunks; c += G)
-            d[c] = shift16(__ldg(s4 + c), __ldg(s4 + c + 1), mis);
-    }
-    for (long long c = head + chunks * 16 + lane; c < len; c += G)
-        dst[c] = src[c];
-}
-
 template <int G>
 __global__ void __launch_bounds__(256) k_list_str_gather(const unsigned long long *vals, const unsigned long long *starts, const long long *off,
                                                          unsigned long long total, const char *pool, char *out, uint8_t *valid) {

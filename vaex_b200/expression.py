@@ -321,7 +321,7 @@ class DeviceExpression:
             elif hasattr(v, "__cuda_array_interface__") and not isinstance(v, np.ndarray):
                 dtypes[k] = np.dtype(v.__cuda_array_interface__["typestr"])
             else:
-                dtypes[k] = v.dtype
+                dtypes[k] = getattr(v, "dtype", np.dtype("O"))  # arrow string columns (a join's gathered strings) have no numpy dtype
         self.program = Program(expression, dtypes, variables)
         self.dtype = self.program.dtype
         self.columns = [columns[name] for name in self.program.inputs]  # the executor looks here to decide host / device feeding

@@ -646,6 +646,23 @@ class Frame:
         keys, _ = self.value_counts(expression, dropna=dropna)
         return keys
 
+    # ---- join: the right's index, the left's lookup and the row gathers on the device (vaex_b200/join.py) ----------------------
+    def _index(self, expression, prime_growth=False, cardinality=None):
+        """df._index (vaex/dataframe.py:514-572): the device index_hash_<T> of `expression` over the frame's rows"""
+        from . import join as _join
+        return _join.index(self, str(expression))
+
+    def join(self, other, on=None, left_on=None, right_on=None, lprefix='', rprefix='', lsuffix='', rsuffix='', how='left', allow_duplication=False,
+             prime_growth=False, cardinality_other=None, inplace=False):
+        """df.join (vaex/join.py:125-297): `other`'s columns added to this frame's rows by the key `on` (or `left_on` / `right_on`:
+        columns or expressions of numeric or datetime dtype), or side by side without a key.  how = 'left', 'right' or 'inner'; a
+        right side with duplicate keys raises unless allow_duplication=True, and then repeats the left's rows, appended in (left row,
+        right row) order.  The gathered columns land where the left key lives (torch on the device, numpy on the host; strings as
+        arrow); a column with a missing row is a host np.ma array.  `prime_growth` and `cardinality_other` are ignored."""
+        from . import join as _join
+        return _join.join(self, other, on=on, left_on=left_on, right_on=right_on, lprefix=lprefix, rprefix=rprefix, lsuffix=lsuffix, rsuffix=rsuffix,
+                          how=how, allow_duplication=allow_duplication, prime_growth=prime_growth, cardinality_other=cardinality_other, inplace=inplace)
+
     # ---- groupby ------------------------------------------------------------------------------------------------------
     def groupby(self, by, agg=None, sort=False, fused=True, combine=False):
         gb = GroupBy(self, by, sort=sort, fused=fused, combine=combine)

@@ -339,9 +339,11 @@ class _IndexHash:
 
     # -- reference protocol --------------------------------------------------------------------------
     def update(self, values, *args, **kwargs):
-        """update(values[, masks], start_index=0, chunk_size=..., bucket_size=..., return_values=False)"""
+        """update(values[, masks], start_index=0, chunk_size=..., bucket_size=..., return_values=False); the keyword `slot` (this
+        project's addition) names the context slot whose stream the call runs on, so the executor's threads update one index at once"""
         names = ["start_index", "chunk_size", "bucket_size", "return_values"]
         masks = kwargs.pop("masks", None)
+        slot = int(kwargs.pop("slot", 0))
         args = list(args)
         if args and not isinstance(args[0], (int, np.integer, bool)):
             masks = args.pop(0)
@@ -360,7 +362,7 @@ class _IndexHash:
             mcol = _lib.mask_column(masks)
             if mcol.length != col.length:
                 raise RuntimeError("array and mask should be of same size")
-        _lib.check(_lib.lib().b200_index_update(self._h, 0, col.ptr, None if mcol is None else mcol.ptr, col.length, int(opts["start_index"]),
+        _lib.check(_lib.lib().b200_index_update(self._h, slot, col.ptr, None if mcol is None else mcol.ptr, col.length, int(opts["start_index"]),
                                                 _lib.memspace(col, mcol), 0))
 
     def merge(self, other):
@@ -370,7 +372,7 @@ class _IndexHash:
         arr = (C.c_void_p * len(others))(*[o._h for o in others])
         _lib.check(_lib.lib().b200_index_merge(self._h, arr, len(others)))
 
-    def _map(self, values, mask, out):
+    def _map(self, values, mask, out, slot=0):
         col = self._lookup_column(values)
         mcol = None if mask is None else _lib.mask_column(mask)
         if mcol is not None and mcol.length != col.length:
@@ -387,28 +389,28 @@ class _IndexHash:
             raise TypeError(f"map_index: out must be an int8, int16, int32 or int64 array of at least {col.length} rows")
         unknown = C.c_int32(0)
         if col.length:
-            _lib.check(_lib.lib().b200_index_map(self._h, 0, col.ptr, None if mcol is None else mcol.ptr, col.length, ocol.ptr, _INDEX_OUT[ocol.dtype],
+            _lib.check(_lib.lib().b200_index_map(self._h, slot, col.ptr, None if mcol is None else mcol.ptr, col.length, ocol.ptr, _INDEX_OUT[ocol.dtype],
                                                  C.byref(unknown), _lib.memspace(col, mcol, ocol), 0))
         if isinstance(out, np.ndarray) and ocol.keep is not out:
             out[:] = ocol.keep  # a non-contiguous host `out` was written through a copy
         return out if give else bool(unknown.value)
 
-    def map_index(self, values, out=None):
+    def map_index(self, values, out=None, slot=0):
         """map_index(values) -> int64 rows (-1: not found); map_index(values, out) writes int8..int64 ``out`` (truncating) and returns
         whether a key was not found"""
-        return self._map(values, None, out)
+        return self._map(values, None, out, slot)
 
-    def map_index_masked(self, values, mask, out=None):
-        return self._map(values, mask, out)
+    def map_index_masked(self, values, mask, out=None, slot=0):
+        return self._map(values, mask, out, slot)
 
-    def map_index_duplicates(self, values, start_index, mask=None, device=False):
+    def map_index_duplicates(self, values, start_index, mask=None, device=False, slot=0):
         """(left rows, right rows): for every row i of `values` whose key has an overflow, ``start_index + i`` paired with each overflow
         row.  `mask` (masked rows contribute none) and `device` (torch results on the index's GPU) are this project's additions."""
         col = self._lookup_column(values)
         mcol = None if mask is None else _lib.mask_column(mask)
         lib, ms = _lib.lib(), _lib.memspace(col, mcol)
         total = C.c_int64(0)
-        args = (self._h, 0, col.ptr, None if mcol is None else mcol.ptr, col.length, int(start_index))
+        args = (self._h, slot, col.ptr, None if mcol is None else mcol.ptr, col.length, int(start_index))
         _lib.check(lib.b200_index_duplicates(*args, None, None, 0, C.byref(total), ms, 0))
         while True:  # the pairs are written only when they fit: an update from another thread in between changes the total
             n = total.value

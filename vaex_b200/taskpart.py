@@ -339,6 +339,93 @@ class TaskPartHashmapUniqueCreate(TaskPart):
         return self.hash_map_unique._internal.__sizeof__()
 
 
+def _key_block(block):
+    """a join key block -> (keys, mask or None): datetimes and timedeltas travel as int64 (vaex/join.py:192-193)"""
+    if _is_device(block):
+        return block, None
+    mask = None
+    if np.ma.isMaskedArray(block):
+        block, mask = np.ascontiguousarray(block.data), np.ma.getmaskarray(block)
+    block = np.asarray(block)
+    return (block.view(np.int64) if block.dtype.kind in "mM" else block), mask
+
+
+class TaskPartIndex(TaskPart):
+    """DataFrame._index (vaex/dataframe.py:514-572): ONE device index_hash_<T> for the pass; every thread updates it on its own slot
+    with its chunk's global rows.  The index follows the sequential rule whatever the thread count and chunk order, so the reference's
+    per-thread indices and their merge (:540-571) have nothing to do here."""
+
+    def __init__(self, expression, dtype, nmaps=1):
+        self.expression = str(expression)
+        self.expressions = [self.expression]
+        self.index = _hash.index_type_from_dtype(dtype)(nmaps)
+        self._ctx = _lib.context()
+
+    def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
+        assert filter_mask is None, "the indexed side of a join is extracted first: its rows are its unfiltered rows"
+        keys, mask = _key_block(blocks[0])
+        self.index.update(keys, masks=mask, start_index=i1, slot=self._ctx.slot(thread_index))
+
+    def reduce(self, others):
+        pass
+
+    def get_result(self):
+        return self.index
+
+
+class TaskPartLookup(TaskPart):
+    """The lookup pass of vaex/join.py:185-209 over every unfiltered row of the left key (run without the filter): map_index /
+    map_index_masked into `lookup[i1:i2]` (host or device), and with duplicates on the right map_index_duplicates, kept on the
+    device.  Result: (whether a row found nothing, [(i1, left rows, right rows)] in row order)."""
+
+    def __init__(self, index, expression, lookup, duplicates):
+        import threading
+        self.index = index
+        self.expression = str(expression)
+        self.expressions = [self.expression]
+        self.lookup = lookup
+        self.duplicates = duplicates
+        self.unknown = False
+        self.extra = []
+        self._lock = threading.Lock()
+        self._ctx = _lib.context()
+
+    def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
+        keys, mask = _key_block(blocks[0])
+        native = self.index._np_dtype()
+        if _is_device(keys) and np.dtype(keys.__cuda_array_interface__["typestr"]) != native:
+            keys = _device_cast(keys, native, self._ctx)
+        slot = self._ctx.slot(thread_index)
+        out = self.lookup[i1:i2]
+        if mask is None:
+            unknown = self.index.map_index(keys, out, slot=slot)
+        else:
+            unknown = self.index.map_index_masked(keys, mask, out, slot=slot)
+        extra = self.index.map_index_duplicates(keys, i1, mask, device=True, slot=slot) if self.duplicates else None
+        with self._lock:
+            self.unknown = self.unknown or bool(unknown)
+            if extra is not None and len(extra[0]):
+                self.extra.append((i1,) + tuple(extra))
+
+    def reduce(self, others):
+        self.extra.sort(key=lambda e: e[0])
+
+    def get_result(self):
+        return self.unknown, self.extra
+
+
+def _device_cast(keys, dtype, ctx):
+    """a device key column of another dtype as `dtype`, where numpy would cast it safely (map_index refuses the rest)"""
+    import torch
+    have = np.dtype(keys.__cuda_array_interface__["typestr"])
+    if not np.can_cast(have, dtype, "safe"):
+        raise TypeError(f"map_index: incompatible key dtype {have} (index dtype {dtype})")
+    ctx.sync()  # a device expression's block is written on a slot's stream
+    out = torch.as_tensor(keys, device=f"cuda:{ctx.device}").to(getattr(torch, dtype.name))
+    torch.cuda.synchronize(out.device)  # the cast runs on torch's stream, the lookup on a slot's
+    return out
+
+
 class TaskPartStatistic(TaskPart):
     """vaex/cpu.py:487-626 — the legacy statistics (df.cov, df.correlation, binned df.minmax, the limits pre-pass) on one device
     grid per compute class (csrc/statistic.cu).  ``blocks`` are the binby blocks followed by the weight blocks."""

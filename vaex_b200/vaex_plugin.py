@@ -16,6 +16,7 @@ task spec's ``task-type`` to ``task-part-cpu-type`` and calls ``encoding.decode(
 import numpy as np
 
 from . import agg as _agg
+from . import hash as _hash
 from . import taskpart as _tp
 
 
@@ -89,12 +90,26 @@ class VaexTaskPartStatistic(_tp.TaskPartStatistic):
 
 
 _ORIGINAL = {}
+_ORIGINAL_INDEX = []  # vaex.hash.index_type_from_dtype, while the device classes stand in for it
 
 
-def install(legacy_statistic=False):
+def device_index_type_from_dtype(dtype, transient=True, prime_growth=False):
+    """vaex.hash.index_type_from_dtype with the device index_hash_<T> for numeric and datetime keys; string keys keep vaex's own"""
+    try:
+        return _hash.index_type_from_dtype(getattr(dtype, "numpy", dtype))
+    except TypeError:
+        return _ORIGINAL_INDEX[0](dtype, transient, prime_growth)
+
+
+def install(legacy_statistic=False, index_hash=False):
     """Swap the two task parts in vaex's registry — and with ``legacy_statistic=True`` also "legacy_statistic" (TaskStatistic);
-    returns the replaced classes so `uninstall` can restore them."""
+    returns the replaced classes so `uninstall` can restore them.  ``index_hash=True`` points vaex.hash.index_type_from_dtype at the
+    device index classes, so vaex's own df.join (vaex/join.py, with host lookups) and df._index run on the device index."""
     import vaex.cpu
+    if index_hash and not _ORIGINAL_INDEX:
+        import vaex.hash
+        _ORIGINAL_INDEX.append(vaex.hash.index_type_from_dtype)
+        vaex.hash.index_type_from_dtype = device_index_type_from_dtype
     _ORIGINAL["aggregations"] = vaex.cpu.TaskPartAggregation
     _ORIGINAL["hash_map_unique_create"] = vaex.cpu.TaskPartHashmapUniqueCreate
     vaex.cpu.register(VaexTaskPartAggregation)
@@ -110,3 +125,6 @@ def uninstall():
     for cls in _ORIGINAL.values():
         vaex.cpu.register(cls)
     _ORIGINAL.clear()
+    if _ORIGINAL_INDEX:
+        import vaex.hash
+        vaex.hash.index_type_from_dtype = _ORIGINAL_INDEX.pop()
