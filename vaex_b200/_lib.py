@@ -284,6 +284,52 @@ def context(device=None):
 # ------------------------------------------------------------------------------------------------
 # column marshalling: numpy arrays are host buffers, anything with __cuda_array_interface__ is device memory
 # ------------------------------------------------------------------------------------------------
+def is_device(x):
+    return hasattr(x, "__cuda_array_interface__") and not isinstance(x, np.ndarray)
+
+
+def on_device(col):
+    """whether a column's chunks are device memory: a device-evaluated virtual column (expression.DeviceExpression,
+    hash.CombinedCodes) when every one of its inputs is, so also one without inputs"""
+    if getattr(col, "device_virtual", False):
+        return all(is_device(c) for c in col.columns)
+    return is_device(col)
+
+
+def chunk_of(col, thread_index, i1, i2):
+    """rows [i1, i2) of a column; a device-evaluated virtual column is evaluated on the slot of `thread_index`"""
+    return col.chunk(thread_index, i1, i2) if getattr(col, "device_virtual", False) else col[i1:i2]
+
+
+def dtype_of(col):
+    """the numpy dtype of a column: object for strings, the typestr of device memory, the data's dtype of a masked array"""
+    from .hash import is_string_column
+    if is_string_column(col):
+        return np.dtype("O")
+    if getattr(col, "device_virtual", False):
+        return col.dtype
+    if is_device(col):
+        return np.dtype(col.__cuda_array_interface__["typestr"])
+    return col.dtype if np.ma.isMaskedArray(col) else np.asarray(col).dtype
+
+
+def split_mask(block):
+    """a block -> (data, mask or None): a host np.ma block gives its contiguous data and its mask (1 = masked)"""
+    if not is_device(block) and np.ma.isMaskedArray(block):
+        return np.ascontiguousarray(block.data), np.ma.getmaskarray(block)
+    return block, None
+
+
+def unmask_selection(mask):
+    """vaex.utils.unmask_selection_mask: a host selection mask as an array in which the masked rows are not selected; device
+    masks pass through"""
+    if is_device(mask):
+        return mask
+    if np.ma.isMaskedArray(mask):
+        return np.asarray(mask.data & ~np.ma.getmaskarray(mask))
+    return np.asarray(mask)
+
+
 class Column:
     __slots__ = ("ptr", "memspace", "dtype", "code", "byteswap", "length", "keep")
 
@@ -300,8 +346,8 @@ def _np_dtype_code(dt):
 
 def column(ar, expected_itemsize=None):
     c = Column()
-    cai = getattr(ar, "__cuda_array_interface__", None)
-    if cai is not None and not isinstance(ar, np.ndarray):
+    if is_device(ar):
+        cai = ar.__cuda_array_interface__
         shape = cai["shape"]
         if len(shape) != 1:
             raise RuntimeError("Expected a 1d array")
@@ -343,8 +389,7 @@ def memspace(*columns):
 
 def mask_column(ar):
     """uint8/bool mask -> Column (bool viewed as uint8)."""
-    cai = getattr(ar, "__cuda_array_interface__", None)
-    if cai is not None and not isinstance(ar, np.ndarray):
+    if is_device(ar):
         c = column(ar)
         if c.dtype.itemsize != 1:
             raise RuntimeError("masks must be 1 byte per row")

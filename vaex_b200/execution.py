@@ -18,11 +18,8 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
+from . import _lib
 from . import taskpart as _tp
-
-
-def _is_device(x):
-    return hasattr(x, "__cuda_array_interface__") and not isinstance(x, np.ndarray)
 
 
 class Task:
@@ -78,18 +75,10 @@ class Executor:
             if declared is not None and declared != t.part.memory_usage():
                 raise RuntimeError(f"Reported memory usage by tasks was {t.part.memory_usage()}, while tracker listed {declared}")
 
-        def on_device(col):
-            if getattr(col, "device_virtual", False):
-                return all(_is_device(c) for c in col.columns)
-            return _is_device(col)
         feed_cols = [columns[e] for e in needed] + ([filter] if filter is not None else []) + [s for t in tasks for s in t.selections if s is not None]
-        device = bool(feed_cols) and all(on_device(c) for c in feed_cols)
+        device = bool(feed_cols) and all(_lib.on_device(c) for c in feed_cols)
         errors = []
         cancelled = threading.Event()
-
-        def block_of(col, thread_index, i1, i2):
-            # virtual columns evaluated on the device (hash.CombinedCodes, expression.DeviceExpression) are produced on this worker's slot
-            return col.chunk(thread_index, i1, i2) if getattr(col, "device_virtual", False) else col[i1:i2]
 
         def feed(thread_index, i1, i2):
             if cancelled.is_set():
@@ -98,8 +87,8 @@ class Executor:
             for t in tasks:
                 if t.part.stopped:
                     t.stopped = True
-            raw = {e: block_of(columns[e], thread_index, i1, i2) for e in sorted({e for t in live for e in t.expressions})}
-            sels = {id(s): block_of(s, thread_index, i1, i2) for t in live for s in t.selections if s is not None}
+            raw = {e: _lib.chunk_of(columns[e], thread_index, i1, i2) for e in sorted({e for t in live for e in t.expressions})}
+            sels = {id(s): _lib.chunk_of(s, thread_index, i1, i2) for t in live for s in t.selections if s is not None}
             filter_mask = None
             if filter is not None and live:
                 from . import expression as _expr
@@ -159,12 +148,10 @@ class Executor:
 
 def _as_u8(mask):
     """selection masks travel as one byte per row"""
-    if _is_device(mask):
+    mask = _lib.unmask_selection(mask)
+    if _lib.is_device(mask):
         return mask
-    m = np.asarray(mask)
-    if np.ma.isMaskedArray(mask):  # vaex.utils.unmask_selection_mask
-        m = mask.data & ~np.ma.getmaskarray(mask)
-    return np.ascontiguousarray(m).astype(np.bool_, copy=False).view(np.uint8)
+    return np.ascontiguousarray(mask).astype(np.bool_, copy=False).view(np.uint8)
 
 
 class UserAbort(Exception):

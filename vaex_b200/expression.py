@@ -314,14 +314,8 @@ class DeviceExpression:
     def __init__(self, expression, columns, variables=None):
         self.expression = str(expression)
         self._columns = columns
-        dtypes = {}
-        for k, v in columns.items():
-            if getattr(v, "device_virtual", False):
-                dtypes[k] = v.dtype
-            elif hasattr(v, "__cuda_array_interface__") and not isinstance(v, np.ndarray):
-                dtypes[k] = np.dtype(v.__cuda_array_interface__["typestr"])
-            else:
-                dtypes[k] = getattr(v, "dtype", np.dtype("O"))  # arrow string columns (a join's gathered strings) have no numpy dtype
+        # an arrow column has no numpy dtype, so no device expression reads it (a join's gathered strings are arrow)
+        dtypes = {k: _lib.dtype_of(v) if hasattr(v, "dtype") else np.dtype("O") for k, v in columns.items()}
         self.program = Program(expression, dtypes, variables)
         self.dtype = self.program.dtype
         self.columns = [columns[name] for name in self.program.inputs]  # the executor looks here to decide host / device feeding

@@ -17,20 +17,6 @@ from . import execution, taskpart
 from . import hash as _hash
 
 
-def _is_device(x):
-    return hasattr(x, "__cuda_array_interface__") and not isinstance(x, np.ndarray)
-
-
-def _dtype_of(ar):
-    if _hash.is_string_column(ar):
-        return np.dtype("O")
-    if getattr(ar, "device_virtual", False):  # device-evaluated virtual column (hash.CombinedCodes)
-        return ar.dtype
-    if _is_device(ar):
-        return np.dtype(ar.__cuda_array_interface__["typestr"])
-    return np.asarray(ar).dtype if not np.ma.isMaskedArray(ar) else ar.dtype
-
-
 class Frame:
     def __init__(self, columns, nthreads=None, executor=None, categories=None, pin=False, filter=None, variables=None):
         """pin=True page-locks the host (numpy) columns once so that chunk uploads run at PCIe rate (b200_host_register).
@@ -53,6 +39,37 @@ class Frame:
 
     def __len__(self):
         return self.length
+
+    def _derive(self, columns, filter=None):
+        """a frame over `columns` with this frame's executor, categories, variables and, unless `filter` is given, its filter; the
+        filter is compiled again because a compiled expression is bound to its frame's column dict"""
+        return Frame(columns, executor=self.executor, categories=self.categories, filter=self._filter_expression if filter is None else filter,
+                     variables=self.variables)
+
+    def _with_columns(self, names):
+        """this frame when every name is one of its columns, else a derived frame in which each missing name is a device-evaluated
+        column"""
+        missing = [e for e in dict.fromkeys(names) if e not in self.columns]
+        if not missing:
+            return self
+        f = self._derive(self.columns)
+        for e in missing:
+            f.columns[e] = f.expression(e)
+        return f
+
+    def _selection(self, selection):
+        """a selection argument -> None for None / False, a boolean device expression for a string, a mask array as it is, and a
+        list of selections element by element"""
+        if isinstance(selection, (list, tuple)):
+            return [self._selection(one) for one in selection]
+        if selection is None or selection is False:
+            return None
+        if isinstance(selection, str):
+            mask = self.expression(selection)
+            if mask.dtype != np.bool_:
+                raise ValueError("a selection must be a boolean expression")
+            return mask
+        return selection
 
     # ---- expressions: virtual columns, filters, selections — evaluated on the device (csrc/expr.cu) ----------------------------
     def expression(self, text):
@@ -83,9 +100,7 @@ class Frame:
 
     def filter(self, expression):
         """df[df.<expression>]: a filtered view over the same columns (filters combine with &, dataframe.py:5535-5560)"""
-        combined = expression if self._filter_expression is None else f"({self._filter_expression}) & ({expression})"
-        f = Frame(self.columns, executor=self.executor, categories=self.categories, filter=combined, variables=self.variables)
-        return f
+        return self._derive(self.columns, expression if self._filter_expression is None else f"({self._filter_expression}) & ({expression})")
 
     def evaluate(self, expression):
         """host copy of an expression's values over the whole frame (unfiltered), chunked like every other pass"""
@@ -98,7 +113,7 @@ class Frame:
         return self.columns[name]
 
     def dtypes(self):
-        return {k: _dtype_of(v) for k, v in self.columns.items()}
+        return {k: _lib.dtype_of(v) for k, v in self.columns.items()}
 
     def categorize(self, name, min_value=0, count=None):
         """Mark an integer column as ordinal codes [min_value, min_value+count) -> BinnerOrdinal (dataframe.py:5605-5631)."""
@@ -111,35 +126,17 @@ class Frame:
     def _statistic(self, op, binby, weights, limits, shape, selection, edges=False):
         """TaskStatistic(self, binby, shape, limits, weights=weights, op=op, selection=selection) (vaex/tasks.py:431-470), run
         through the executor; returns the reduced grid (one per selection when `selection` is a list)"""
-        binby = [] if binby is None else ([binby] if isinstance(binby, str) else list(binby))
-        shape = [shape] * len(binby) if np.isscalar(shape) else list(shape)
-        if limits is None or isinstance(limits, str):
-            limits = [None] * len(binby)
-        limits = list(limits)
-        if len(binby) == 1 and len(limits) == 2 and np.isscalar(limits[0]):
-            limits = [limits]
+        binby, shape, limits = _binned_args(binby, shape, limits)
         limits = [self.minmax(b).astype("float64") if lim is None else lim for b, lim in zip(binby, limits)]
         waslist = isinstance(selection, (list, tuple))
-        selections = list(selection) if waslist else [selection]
-        masks = []
-        for one in selections:
-            if one is None or one is False:
-                masks.append(None)
-                continue
-            m = self.expression(one)
-            if m.dtype != np.bool_:
-                raise ValueError("a selection must be a boolean expression")
-            masks.append(m)
+        masks = self._selection(selection) if waslist else [self._selection(selection)]
         part = taskpart.TaskPartStatistic(self, [int(s) + 3 if edges else int(s) for s in shape], binby, np.dtype("f8"),
                                           [None if m is None else "selection%d" % i for i, m in enumerate(masks)], op, list(weights),
                                           [float(lim[0]) for lim in limits], [float(lim[1]) for lim in limits], edges, waslist)
-        columns = dict(self.columns)
-        for e in list(binby) + list(weights):
-            if e not in columns:
-                columns[e] = self.expression(e)
+        f = self._with_columns(binby + list(weights))
         task = execution.Task(part, masks)
-        task.expressions = list(binby) + list(weights)
-        self.executor.execute(columns, [task], self.length, filter=self._filter)
+        task.expressions = binby + list(weights)
+        f.executor.execute(f.columns, [task], f.length, filter=f._filter)
         return task.result
 
     def cov(self, x, y=None, binby=None, limits=None, shape=128, selection=None):
@@ -196,17 +193,13 @@ class Frame:
         expression"""
         single = not isinstance(x, (list, tuple))
         xs, ys = ([x], [y]) if single else (list(x), list(y))
-        binby_l = [] if binby is None else ([binby] if isinstance(binby, str) else list(binby))
+        binby_l = _binned_args(binby, shape, limits)[0]
         if binby_l and (limits is None or isinstance(limits, str)):
             limits = [self.minmax(b).astype("float64") for b in binby_l]
         out = []
         for a, b in zip(xs, ys):
             name = "(%s)*(%s)" % (a, b)
-            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
-            for e in (a, b):
-                if e not in f.columns:
-                    f.columns[e] = f.expression(e)
-            f.columns[name] = f.expression(name)
+            f = self._with_columns([a, b, name])
             kw = dict(binby=binby_l or None, limits=limits, shape=shape, selection=selection)
             mx, my, mxy = f._agg([_agg.mean(a), _agg.mean(b), _agg.mean(name)], **kw)
             out.append(mxy - mx * my)
@@ -226,9 +219,7 @@ class Frame:
             if raw:
                 return res
             col = self.columns.get(expression)
-            dt = np.dtype(_dtype_of(col) if col is not None else self.expression(expression).dtype).newbyteorder("=")
-            with np.errstate(invalid="ignore"):
-                return res if dt.kind in "mM" else res.astype(dt)
+            return _minmax_as(res, _lib.dtype_of(col) if col is not None else self.expression(expression).dtype)
         import ctypes as C
         col = self.columns[expression]
         ctx = _lib.context()
@@ -237,12 +228,12 @@ class Frame:
             # virtual columns and filtered frames: evaluate / compact chunk by chunk on the device, reduce every chunk
             from . import expression as _expr
             lo, hi, dt = np.inf, -np.inf, None
-            chunk = max(self.executor.chunk_size_for(self.length), 1) if not all(_is_device(c) for c in getattr(col, "columns", [col])) else max(self.length, 1)
+            chunk = max(self.executor.chunk_size_for(self.length), 1) if not _lib.on_device(col) else max(self.length, 1)
             for i1 in range(0, self.length, chunk):
                 i2 = min(i1 + chunk, self.length)
-                block = col.chunk(0, i1, i2) if getattr(col, "device_virtual", False) else col[i1:i2]
+                block = _lib.chunk_of(col, 0, i1, i2)
                 if self._filter is not None:
-                    if not _is_device(block) and np.ma.isMaskedArray(block):
+                    if not _lib.is_device(block) and np.ma.isMaskedArray(block):
                         raise NotImplementedError("minmax of a masked column on a filtered frame")
                     kept, (block,) = _expr.compact(0, self._filter.chunk(0, i1, i2), [block], ctx)
                     if not kept:
@@ -252,25 +243,13 @@ class Frame:
                 _lib.check(_lib.lib().b200_minmax(ctx._h, 0, c.code, c.byteswap, c.ptr, None, c.length, c.memspace, out))
                 lo, hi = min(lo, out[0]), max(hi, out[1])
             res = np.array([lo, hi])
-            if raw:
-                return res
-            dt = np.dtype(dt if dt is not None else _dtype_of(col)).newbyteorder("=")
-            with np.errstate(invalid="ignore"):
-                return res if dt.kind in "mM" else res.astype(dt)
-        mask = None
-        if not _is_device(col) and np.ma.isMaskedArray(col):
-            mask = _lib.mask_column(np.ma.getmaskarray(col))
-            col = np.ascontiguousarray(col.data)
+            return res if raw else _minmax_as(res, dt if dt is not None else _lib.dtype_of(col))
+        col, mask = _lib.split_mask(col)
+        mask = None if mask is None else _lib.mask_column(mask)
         c = _lib.column(col)
         _lib.check(_lib.lib().b200_minmax(ctx._h, 0, c.code, c.byteswap, c.ptr, None if mask is None else mask.ptr, c.length, c.memspace, out))
         res = np.array([out[0], out[1]])
-        if raw:
-            return res
-        dt = np.dtype(c.dtype).newbyteorder("=")
-        if dt.kind in "mM":
-            return res
-        with np.errstate(invalid="ignore"):
-            return res.astype(dt)
+        return res if raw else _minmax_as(res, c.dtype)
 
     def limits(self, expressions, value="minmax", selection=None):
         """df.limits (vaex/dataframe.py:1844-2004): the (min, max) pair `value` describes per expression: "minmax", "N%"
@@ -340,33 +319,19 @@ class Frame:
         percentile_shapes = _expand_shape(percentile_shape, len(expressions))
         if percentile_limits:
             percentile_limits = _expand_limits(percentile_limits, len(expressions))
-        f = self
-        missing = [e for e in expressions + binby if e not in self.columns]
-        if missing:
-            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
-            for e in missing:
-                f.columns[e] = f.expression(e)
+        f = self._with_columns(expressions + binby)
         for e in expressions + binby:
-            if e in f.categories or _dtype_of(f.columns[e]).kind in "mM":
+            if e in f.categories or _lib.dtype_of(f.columns[e]).kind in "mM":
                 raise NotImplementedError(f"percentile_approx over the categorical or datetime column {e!r} is not supported")
         binby_limits = f._limits_list(binby, limits, selection)
         expression_limits = f._limits_list(expressions, percentile_limits, selection)
-        mask = f.expression(selection) if isinstance(selection, str) else selection
-        if isinstance(selection, str) and mask.dtype != np.bool_:
-            raise ValueError("a selection must be a boolean expression")
+        mask = f._selection(selection)
         dtypes = f.dtypes()
-        nthreads = f.executor.nthreads
-
-        def spec(e, count, lim):
-            return {"binner-type": "scalar", "expression": e, "dtype": dtypes[e].str, "count": int(count), "minimum": float(lim[0]),
-                    "maximum": float(lim[1])}
         tasks = []
         for e, pshape, plim in zip(expressions, percentile_shapes, expression_limits):
-            specs = [spec(b, n, lim) for b, n, lim in zip(binby, shape, binby_limits)] + [spec(e, pshape, plim)]
-            desc = _agg.count("*", selection=None if mask is None else "selection", edges=True)
-            desc._prepare_types(dtypes)
-            part = taskpart.TaskPartPercentile(None, [taskpart.decode_binner(s, nthreads) for s in specs], [desc], dtypes, plim, percentage,
-                                               nthreads=nthreads)
+            specs = [_scalar_spec(b, dtypes[b], n, lim) for b, n, lim in zip(binby, shape, binby_limits)]
+            specs.append(_scalar_spec(e, dtypes[e], pshape, plim))
+            part = taskpart.TaskPartCountGrid("percentile_approx", specs, mask is not None, dtypes, _pct.finish, (plim, percentage), f.executor.nthreads)
             tasks.append(execution.Task(part, [mask]))
         f.executor.execute(f.columns, tasks, f.length, filter=f._filter)
         return _pct.unlistify(waslist, np.array([t.result for t in tasks]))
@@ -392,38 +357,25 @@ class Frame:
         if len(binby) > 3:
             raise ValueError("binby with dim > 3 is not yet supported")
         binby = [str(b) for b in binby]
-        selection = None if selection is False else selection
         binby_shape = _expand_shape(shape, len(binby))
         combinations_unique, unique_reverse = _mi.unique_combinations(combinations)
-        f = self
         names = list(dict.fromkeys([str(e) for c in combinations_unique for e in c] + binby))
-        missing = [e for e in names if e not in self.columns]
-        if missing:
-            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
-            for e in missing:
-                f.columns[e] = f.expression(e)
+        f = self._with_columns(names)
         for e in names:
-            if e in f.categories or _dtype_of(f.columns[e]).kind in "mMO":
+            if e in f.categories or _lib.dtype_of(f.columns[e]).kind in "mMO":
                 raise NotImplementedError(f"mutual_information over the categorical, datetime or string column {e!r} is not supported")
         # the limits come from all rows of the frame, not the selection's (:762, :769), and every name's minmax once per call
         memo = {}
         binby_limits = f._limits_list(binby, limits, None, memo)
         values = _per_expression(mi_limits, len(combinations_unique))
         combination_limits = [f._limits_list([str(e) for e in c], v, None, memo) for c, v in zip(combinations_unique, values)]
-        mask = f.expression(selection) if isinstance(selection, str) else selection
-        if isinstance(selection, str) and mask.dtype != np.bool_:
-            raise ValueError("a selection must be a boolean expression")
+        mask = f._selection(selection)
         dtypes = f.dtypes()
-        nthreads = f.executor.nthreads
-
-        def spec(e, count, lim):
-            return {"binner-type": "scalar", "expression": e, "dtype": dtypes[e].str, "count": int(count), "minimum": float(lim[0]),
-                    "maximum": float(lim[1])}
         plans = []
         for c, lims in zip(combinations_unique, combination_limits):
             c = [str(e) for e in c]
-            specs = [spec(e, n, lim) for e, n, lim in zip(c, _expand_shape(mi_shape, len(c)), lims)]
-            specs += [spec(b, n, lim) for b, n, lim in zip(binby, binby_shape, binby_limits)]
+            specs = [_scalar_spec(e, dtypes[e], n, lim) for e, n, lim in zip(c, _expand_shape(mi_shape, len(c)), lims)]
+            specs += [_scalar_spec(b, dtypes[b], n, lim) for b, n, lim in zip(binby, binby_shape, binby_limits)]
             plans.append((len(c), specs, 8 * int(np.prod([s["count"] + 3 for s in specs], dtype=np.int64))))
         budget, free = _mi.grid_budget(_lib.context().device)
         for (_, specs, nbytes), c in zip(plans, combinations_unique):
@@ -436,10 +388,7 @@ class Frame:
             tasks = []
             for i in batch:
                 d, specs, _ = plans[i]
-                desc = _agg.count("*", selection=None if mask is None else "selection", edges=True)
-                desc._prepare_types(dtypes)
-                part = taskpart.TaskPartMutualInformation(None, [taskpart.decode_binner(s, nthreads) for s in specs], [desc], dtypes, d,
-                                                          nthreads=nthreads)
+                part = taskpart.TaskPartCountGrid("mutual_information", specs, mask is not None, dtypes, _mi.finish, (d,), f.executor.nthreads)
                 tasks.append(execution.Task(part, [mask]))
             f.executor.execute(f.columns, tasks, f.length, filter=f._filter)
             mi_list += [t.result for t in tasks]
@@ -457,23 +406,15 @@ class Frame:
         binby = [str(b) for b in ([binby] if isinstance(binby, str) else list(binby))]
         expression = str(expression)
         shape = _mode.grid_shape(binby, shape, mode_shape)
-        selection = None if selection is False else selection
-        f = self
         names = list(dict.fromkeys(binby + [expression]))
-        missing = [e for e in names if e not in self.columns]
-        if missing:
-            f = Frame(dict(self.columns), executor=self.executor, categories=self.categories, filter=self._filter_expression, variables=self.variables)
-            for e in missing:
-                f.columns[e] = f.expression(e)
+        f = self._with_columns(names)
         for e in names:
-            if _dtype_of(f.columns[e]).kind not in "biuf":
+            if _lib.dtype_of(f.columns[e]).kind not in "biuf":
                 raise NotImplementedError(f"mode over the string, object or datetime column {e!r} is not supported")
         limits = list(f.limits(binby, limits)) + list(f.limits([expression], mode_limits))
         centers = _mode.centers(*limits[-1], mode_shape)
         _mode.check_memory(shape, _lib.context().device)
-        mask = f.expression(selection) if isinstance(selection, str) else selection
-        if isinstance(selection, str) and mask.dtype != np.bool_:
-            raise ValueError("a selection must be a boolean expression")
+        mask = f._selection(selection)
         order = _mode.axis_order(binby + [expression])
         lims = _mode.axis_order(limits)
         part = taskpart.TaskPartMode(None, shape, order, [float(lim[0]) for lim in lims], [float(lim[1]) for lim in lims], centers,
@@ -484,23 +425,13 @@ class Frame:
 
     # ---- binned statistics -------------------------------------------------------------------------------------------
     def _binner_specs(self, binby, limits, shape):
-        if binby is None or binby == []:
-            return []
-        if isinstance(binby, (str, dict)):
-            binby = [binby]
-        nd = len(binby)
-        shapes = [shape] * nd if np.isscalar(shape) else list(shape)
-        if limits is None or isinstance(limits, str):
-            limits = [None] * nd
-        limits = list(limits)
-        if nd == 1 and len(limits) == 2 and np.isscalar(limits[0]):
-            limits = [limits]
+        binby, shapes, limits = _binned_args(binby, shape, limits)
         specs = []
         for i, b in enumerate(binby):
             if isinstance(b, dict):  # explicit spec (ordinal / hash binners)
                 specs.append(b)
                 continue
-            dtype = _dtype_of(self.columns[b])
+            dtype = _lib.dtype_of(self.columns[b])
             if b in self.categories:
                 lo, count = self.categories[b]
                 specs.append({"binner-type": "ordinal", "expression": b, "dtype": dtype.str, "count": count, "minimum": lo, "invert": False})
@@ -508,8 +439,7 @@ class Frame:
             lim = limits[i]
             if lim is None:
                 lim = self.minmax(b).astype("float64")  # the extra pass the reference runs for limits=None (dataframe.py:5618)
-            specs.append({"binner-type": "scalar", "expression": b, "dtype": dtype.str, "count": int(shapes[i]), "minimum": float(lim[0]),
-                          "maximum": float(lim[1])})
+            specs.append(_scalar_spec(b, dtype, shapes[i], lim))
         return specs
 
     def _agg(self, aggregators, binby=None, limits=None, shape=128, selection=None, edges=False, progress=None):
@@ -518,17 +448,8 @@ class Frame:
         aggregators = [aggregators] if single else list(aggregators)
         specs = self._binner_specs(binby, limits, shape)
         dtypes = self.dtypes()
-        def as_mask(one):
-            if isinstance(one, str):  # a selection expression: a boolean mask evaluated on the device per chunk
-                one = self.expression(one)
-                if one.dtype != np.bool_:
-                    raise ValueError("a selection must be a boolean expression")
-            return one
         # a LIST of selections gives one grid per selection, stacked along a new first axis (vaex/cpu.py:744-786, :798-811)
-        if isinstance(selection, (list, tuple)):
-            selection = [None if one is None or one is False else as_mask(one) for one in selection]
-        else:
-            selection = as_mask(selection)
+        selection = self._selection(selection)
         requests = []
         for a in aggregators:
             for prim in a.primitives():
@@ -597,10 +518,10 @@ class Frame:
         does), so masked rows stay out of count / sum / sum_moment."""
         columns = self.columns if columns is None else columns
         col = columns[expression]
-        if _dtype_of(col).kind == "f":
+        if _lib.dtype_of(col).kind == "f":
             return expression  # float32 already accumulates in double: identical result without the cast
         name = f"astype({expression}, 'float64')"
-        if _is_device(col):
+        if _lib.is_device(col):
             columns[name] = col.double()
         elif np.ma.isMaskedArray(col):
             columns[name] = np.ma.array(np.asarray(col.data).astype("float64"), mask=np.ma.getmaskarray(col))
@@ -624,15 +545,15 @@ class Frame:
             order = np.argsort(counts, kind="stable")
             order = order if ascending else order[::-1]
             return keys[order], counts[order]
-        dt = _dtype_of(col)
+        dt = _lib.dtype_of(col)
         counter = getattr(superutils, "counter_" + np.dtype(dt).newbyteorder("=").name)(1)
-        chunk = self.executor.chunk_size_for(self.length) if not _is_device(col) else max(self.length, 1)
+        chunk = self.executor.chunk_size_for(self.length) if not _lib.is_device(col) else max(self.length, 1)
         for i1 in range(0, self.length, chunk):
-            block = col[i1:i1 + chunk]
-            if not _is_device(block) and np.ma.isMaskedArray(block):
-                counter.update(np.ascontiguousarray(block.data), np.ma.getmaskarray(block))
+            data, mask = _lib.split_mask(col[i1:i1 + chunk])
+            if mask is not None:
+                counter.update(data, mask)
             else:
-                counter.update(block if _is_device(block) else np.ascontiguousarray(block))
+                counter.update(data if _lib.is_device(data) else np.ascontiguousarray(data))
         keys, counts = counter.keys(), counter.counts()
         keep = [i for i, k in enumerate(keys)
                 if not ((k is None and (dropna or dropmissing)) or (isinstance(k, float) and k != k and (dropna or dropnan)))]
@@ -683,11 +604,7 @@ class GroupBy:
         (hash.CombinedCodes) and the groupby runs over the distinct codes — the reference's sparse `_combine` path
         (vaex/groupby.py:526-584)."""
         self.by = [by] if isinstance(by, str) else list(by)
-        if any(name not in df.columns for name in self.by):  # a key that is an expression: group by it as a virtual column
-            df = Frame(dict(df.columns), executor=df.executor, categories=df.categories, filter=df._filter_expression, variables=df.variables)
-            for name in self.by:
-                if name not in df.columns:
-                    df.add_virtual_column(name, name)
+        df = df._with_columns(self.by)  # a key that is an expression: group by it as a virtual column
         self.df = df
         self.fused = fused
         self.sort = sort
@@ -695,7 +612,7 @@ class GroupBy:
         self.hash_maps = []
         for name in self.by:
             col = df.columns[name]
-            part = taskpart.TaskPartHashmapUniqueCreate(None, name, _dtype_of(col), nthreads=1)
+            part = taskpart.TaskPartHashmapUniqueCreate(None, name, _lib.dtype_of(col), nthreads=1)
             # nthreads=1 -> 7 shards, chunks fed in row order: the ordinals of the sequential reference run
             task = execution.Task(part)
             ex = execution.Executor(1, chunk_size_max=df.executor.chunk_size_max)
@@ -794,7 +711,7 @@ class GroupBy:
         if self.combined is not None:
             codes, chm = self.combined
             columns[self._COMBINED] = codes
-            frame = Frame(columns, executor=df.executor, categories=df.categories, filter=df._filter_expression, variables=df.variables)
+            frame = df._derive(columns)
             spec = {"binner-type": "hash", "expression": self._COMBINED, "dtype": "<i8", "hash_map_unique": chm}
             grids = frame._agg(descs, binby=[spec], edges=True)
             counts = grids[-1][:-2]
@@ -808,7 +725,7 @@ class GroupBy:
             out["count"] = counts[keep]
             return out
         for name, hm in zip(self.by, self.hash_maps):
-            dtype = _dtype_of(df.columns[name])
+            dtype = _lib.dtype_of(df.columns[name])
             if hm.is_string:
                 cname = f"_ordinal_values({name})"
                 columns[cname] = _hash.StringCodes(df.columns[name], hm)
@@ -819,9 +736,9 @@ class GroupBy:
                 codes = hm.map(df.columns[name])
                 cname = f"_ordinal_values({name})"
                 columns[cname] = codes
-                cdt = _dtype_of(codes)
+                cdt = _lib.dtype_of(codes)
                 specs.append({"binner-type": "ordinal", "expression": cname, "dtype": cdt.str, "count": len(hm), "minimum": 0, "invert": False})
-        frame = Frame(columns, executor=df.executor, categories=df.categories, filter=df._filter_expression, variables=df.variables)
+        frame = df._derive(columns)
         grids = frame._agg(descs, binby=specs, edges=True)
         # _extract_center (vaex/groupby.py:896-977): drop the null / nan edge cells, keep groups with count > 0
         center = tuple(slice(0, -2) for _ in self.by)
@@ -870,6 +787,32 @@ def _expand_limits(limits, dimension):
         assert len(limits) == dimension, "wants to expand shape %r to dimension %d" % (limits, dimension)
         return tuple(limits)
     return (limits,) * dimension
+
+
+def _minmax_as(res, dtype):
+    """the (min, max) doubles cast back to the column's dtype (vaex/dataframe.py:1524-1528); datetimes stay raw doubles"""
+    dt = np.dtype(dtype).newbyteorder("=")
+    if dt.kind in "mM":
+        return res
+    with np.errstate(invalid="ignore"):
+        return res.astype(dt)
+
+
+def _binned_args(binby, shape, limits):
+    """binby, shape and limits of the binned and legacy statistics -> (binby list, one shape per binby, one limit pair or None per
+    binby); None or a string `limits` (whatever it says) leaves every limit to the minmax pass"""
+    binby = [] if binby is None else [binby] if isinstance(binby, (str, dict)) else list(binby)
+    shapes = [shape] * len(binby) if np.isscalar(shape) else list(shape)
+    limits = [None] * len(binby) if limits is None or isinstance(limits, str) else list(limits)
+    if len(binby) == 1 and len(limits) == 2 and np.isscalar(limits[0]):
+        limits = [limits]
+    return binby, shapes, limits
+
+
+def _scalar_spec(expression, dtype, count, limit):
+    """the spec of a BinnerScalar (vaex/dataframe.py:7294-7360)"""
+    return {"binner-type": "scalar", "expression": expression, "dtype": dtype.str, "count": int(count), "minimum": float(limit[0]),
+            "maximum": float(limit[1])}
 
 
 def _is_arrow(x):

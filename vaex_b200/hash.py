@@ -4,7 +4,7 @@ Reference: packages/vaex-core/vaex/hash.py:62-292 (add / merge / flatten / keys 
 null/nan bookkeeping).  String and object keys are out of scope (SURVEY.md 8f row 3)."""
 import numpy as np
 
-from . import superutils
+from . import _lib, superutils
 
 
 def is_string_column(ar):
@@ -90,12 +90,10 @@ class HashMapUnique:
         chunk_size = 1024 * 1024
         if self.is_string:
             return self._internal.update(ar, -1, chunk_size=chunk_size, bucket_size=chunk_size * 4, return_values=return_inverse)
-        is_device = hasattr(ar, "__cuda_array_interface__") and not isinstance(ar, np.ndarray)
-        if not is_device and np.ma.isMaskedArray(ar):
-            mask = np.ma.getmaskarray(ar)
-            data = np.ascontiguousarray(ar.data)
+        data, mask = _lib.split_mask(ar)
+        if mask is not None:
             return self._internal.update(data, mask, -1, chunk_size=chunk_size, bucket_size=chunk_size * 4, return_values=return_inverse)
-        if not is_device:
+        if not _lib.is_device(ar):
             ar = np.ascontiguousarray(ar)
         return self._internal.update(ar, -1, chunk_size=chunk_size, bucket_size=chunk_size * 4, return_values=return_inverse)
 
@@ -241,7 +239,6 @@ class CombinedCodes:
     @property
     def _ctx(self):
         if self._ctx_cached is None:
-            from . import _lib
             self._ctx_cached = _lib.context()
         return self._ctx_cached
 
@@ -255,7 +252,6 @@ class CombinedCodes:
 
     def chunk(self, thread_index, i1, i2):
         import ctypes as C
-        from . import _lib
         n = i2 - i1
         out = self._buffer(thread_index, n)
         if n == 0:
@@ -264,7 +260,7 @@ class CombinedCodes:
         keep, kptr, mptr = [], (C.c_void_p * nk)(), (C.c_void_p * nk)()
         for k, col in enumerate(self.columns):
             # a previous stage's codes (vaex/groupby.py:572-582) are produced on this worker's slot, like every device-virtual column
-            part = col.chunk(thread_index, i1, i2) if getattr(col, "device_virtual", False) else col[i1:i2]
+            part = _lib.chunk_of(col, thread_index, i1, i2)
             mask = None
             if isinstance(part, np.ndarray) and np.ma.isMaskedArray(part):
                 mask = np.ma.getmaskarray(part)

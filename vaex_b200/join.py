@@ -17,10 +17,6 @@ from . import hash as _hash
 MAX_TAKE_COLUMNS = 16  # b200_take's columns per launch
 
 
-def _is_device(x):
-    return hasattr(x, "__cuda_array_interface__") and not isinstance(x, np.ndarray)
-
-
 def _is_virtual(x):
     return getattr(x, "device_virtual", False)
 
@@ -38,12 +34,6 @@ def _device_tensor(x):
     """a device column as a torch tensor (DeviceArray views included)"""
     torch = _torch()
     return x if isinstance(x, torch.Tensor) else torch.as_tensor(x, device=f"cuda:{_lib.context().device}")
-
-
-def _dtype(col):
-    if _is_device(col):
-        return np.dtype(col.__cuda_array_interface__["typestr"])
-    return col.dtype
 
 
 def required_dtype_for_max(n):
@@ -76,7 +66,7 @@ def _staged(x):
     """a column on the device for a gather, as a torch tensor: device columns in place, host ones copied once (bit patterns: datetimes
     and unsigned integers travel as signed integers of their width)"""
     torch = _torch()
-    if _is_device(x):
+    if _lib.is_device(x):
         return _device_tensor(x)
     a = np.ascontiguousarray(x)
     if a.dtype.kind in "mMu" and a.dtype.itemsize > 1:
@@ -113,7 +103,7 @@ def take(index, columns, src_len, device):
         group = columns[k:k + MAX_TAKE_COLUMNS]
         srcs, masks, outs, valids, dtypes = [], [], [], [], []
         for data, mask in group:
-            dt = _dtype(data)
+            dt = _lib.dtype_of(data)
             if not dt.isnative:
                 data, dt = np.asarray(data).astype(dt.newbyteorder("=")), dt.newbyteorder("=")
             if len(data) != src_len:
@@ -189,7 +179,7 @@ def take_strings(index, values):
 
 
 def _to_host(x):
-    if _is_device(x):
+    if _lib.is_device(x):
         _lib.context().sync()
         return _device_tensor(x).cpu().numpy()
     return np.asarray(x)
@@ -204,8 +194,7 @@ def gather(columns, index, src_len, device):
         if _hash.is_string_column(col):
             out[name] = take_strings(index, col)[0]
             continue
-        mask = np.ma.getmaskarray(col) if not _is_device(col) and np.ma.isMaskedArray(col) else None
-        data = col.data if mask is not None else col
+        data, mask = _lib.split_mask(col)
         fixed.append((name, data, mask, device(col)))
         out[name] = None
     for dev in (False, True):
@@ -230,10 +219,10 @@ def _concat(a, b):
             x = x if isinstance(x, pa.Array) else pa.array(np.asarray(x, dtype=object).tolist(), type=pa.large_string())
             return x if pa.types.is_large_string(x.type) else x.cast(pa.large_string())
         return pa.concat_arrays([large(a), large(b)])
-    if _is_device(a) and _is_device(b):
+    if _lib.is_device(a) and _lib.is_device(b):
         return _torch().cat([_device_tensor(a), _device_tensor(b)])
     if np.ma.isMaskedArray(a) or np.ma.isMaskedArray(b):
-        return np.ma.concatenate([np.ma.asarray(_to_host(a) if _is_device(a) else a), np.ma.asarray(b)])
+        return np.ma.concatenate([np.ma.asarray(_to_host(a) if _lib.is_device(a) else a), np.ma.asarray(b)])
     return np.concatenate([_to_host(a), _to_host(b)])
 
 
@@ -241,7 +230,7 @@ def _materialize(frame, name):
     """a virtual column's values over the whole frame (unfiltered), on the device when the frame's columns are"""
     values = frame.evaluate(name)
     col = frame.columns[name]
-    if col.columns and all(_is_device(c) for c in col.columns) and values.dtype.kind not in "mM":
+    if col.columns and _lib.on_device(col) and values.dtype.kind not in "mM":
         return _torch().from_numpy(values).to(f"cuda:{_lib.context().device}")
     return values
 
@@ -253,43 +242,24 @@ def extract(frame):
     if frame._filter is None:
         return Frame(columns, executor=frame.executor, variables=frame.variables)
     rows = np.flatnonzero(frame.evaluate(frame._filter_expression))
-    columns = gather(columns, rows, frame.length, _is_device)
+    columns = gather(columns, rows, frame.length, _lib.is_device)
     return Frame(columns, executor=frame.executor, variables=frame.variables)
-
-
-def _key(frame, expression):
-    """(columns for the pass, the key's name there): a column, or an expression evaluated on the device like GroupBy's keys"""
-    columns = dict(frame.columns)
-    if expression not in columns:
-        columns[expression] = frame.expression(expression)
-    return columns, expression
-
-
-def _key_dtype(col):
-    from .frame import _dtype_of
-    return _dtype_of(col)
 
 
 def index(frame, expression, nmaps=None):
     """DataFrame._index (vaex/dataframe.py:514-572): the device index_hash of `expression` over the frame's rows (its filter is not
     applied: the join extracts the right side first)"""
-    columns, name = _key(frame, expression)
-    dtype = _key_dtype(columns[name])
+    columns = frame._with_columns([expression]).columns  # an expression key is evaluated on the device like GroupBy's keys
+    dtype = _lib.dtype_of(columns[expression])
     try:
-        part = taskpart.TaskPartIndex(name, dtype, nmaps or frame.executor.nthreads)
+        part = taskpart.TaskPartIndex(expression, dtype, nmaps or frame.executor.nthreads)
     except TypeError as e:
-        if dtype.kind in "OUS" or _hash.is_string_column(columns[name]):
+        if dtype.kind in "OUS" or _hash.is_string_column(columns[expression]):
             raise TypeError(f"cannot join on the string key {expression!r}: index_hash_string, the device index for string keys, "
                             "is not available") from e
         raise
     frame.executor.execute(columns, [execution.Task(part)], frame.length)
     return part.index
-
-
-def _key_on_device(col):
-    if _is_virtual(col):
-        return bool(col.columns) and all(_is_device(c) for c in col.columns)
-    return _is_device(col)
 
 
 def _rename_in(text, old, new):
@@ -344,15 +314,16 @@ def join(df, other, on=None, left_on=None, right_on=None, lprefix='', rprefix=''
         if duplicates_right and not allow_duplication:
             raise ValueError('This join will lead to duplication of rows which is disabled, pass allow_duplication=True')
         lookup_dtype = required_dtype_for_max(n_other)
-        columns, name = _key(left, left_on)
-        lookup_device = _key_on_device(columns[name])
+        columns = left._with_columns([left_on]).columns
+        key = columns[left_on]
+        lookup_device = _lib.on_device(key) and not (_is_virtual(key) and not key.columns)  # a key without inputs is looked up on the host
         if lookup_device:
             torch = _torch()
             lookup = torch.full((N,), int(np.iinfo(lookup_dtype).max), dtype=_torch_dtype(lookup_dtype), device=f"cuda:{_lib.context().device}")
             torch.cuda.synchronize(lookup.device)  # the fill runs on torch's stream, map_index writes on a slot's
         else:
             lookup = np.full(N, np.iinfo(lookup_dtype).max, dtype=lookup_dtype)
-        part = taskpart.TaskPartLookup(ix, name, lookup, duplicates_right)
+        part = taskpart.TaskPartLookup(ix, left_on, lookup, duplicates_right)
         left.executor.execute(columns, [execution.Task(part)], N)  # every row, filtered or not (join.py:209 ignore_filter=True)
         _, extra = part.get_result()
         if extra:
@@ -362,7 +333,7 @@ def join(df, other, on=None, left_on=None, right_on=None, lprefix='', rprefix=''
             lookup_right = torch.cat([e[2] for e in extra])
             if not lookup_device:
                 lookup_left, lookup_right = lookup_left.cpu().numpy(), lookup_right.cpu().numpy()
-            repeated = gather(real, lookup_left, N, _is_device)
+            repeated = gather(real, lookup_left, N, _lib.is_device)
             real = {k: _concat(v, repeated[k]) for k, v in real.items()}
             lookup = torch.cat([lookup.to(torch.int64), lookup_right]) if lookup_device else np.concatenate([lookup.astype(np.int64), lookup_right])
         if inner:
@@ -381,7 +352,7 @@ def join(df, other, on=None, left_on=None, right_on=None, lprefix='', rprefix=''
             rows, lookup = _device_tensor(rows)[:kept].clone(), _device_tensor(lookup)[:kept].clone()
             if not lookup_device:
                 rows, lookup = rows.cpu().numpy(), lookup.cpu().numpy()
-            real = gather(real, rows, total, _is_device)
+            real = gather(real, rows, total, _lib.is_device)
 
     # renaming, so all names are unique (join.py:231-255)
     right_cols = dict(right.columns)

@@ -131,11 +131,10 @@ class Statistic:
         keep = []
 
         def column(ar):
-            mask = None
-            if not _is_device(ar) and np.ma.isMaskedArray(ar):
-                mask = _lib.mask_column(np.ma.getmaskarray(ar))
-                ar = np.ascontiguousarray(ar.data)
-            if not _is_device(ar) and np.asarray(ar).dtype.kind in "mM":  # the signed count of units, as numpy's astype(float) reads it
+            ar, mask = _lib.split_mask(ar)
+            if mask is not None:
+                mask = _lib.mask_column(mask)
+            if not _lib.is_device(ar) and np.asarray(ar).dtype.kind in "mM":  # the signed count of units, as numpy's astype(float) reads it
                 ar = np.asarray(ar)
                 ar = ar.view(np.dtype(np.int64).newbyteorder(ar.dtype.byteorder))
             c = _lib.column(ar)
@@ -182,6 +181,3 @@ class Statistic:
         except Exception:
             pass
 
-
-def _is_device(x):
-    return hasattr(x, "__cuda_array_interface__") and not isinstance(x, np.ndarray)

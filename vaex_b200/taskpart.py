@@ -25,8 +25,13 @@ def _issequence(x):
     return isinstance(x, (tuple, list))
 
 
-def _is_device(x):
-    return hasattr(x, "__cuda_array_interface__") and not isinstance(x, np.ndarray)
+def _rows(i1, i2, filter_mask, blocks):
+    """the rows of a chunk the part sees: all of [i1, i2), or those the filter kept when the executor compacted the blocks with it
+    (vaex/execution.py:516-522); count(*) has no block to take that length from"""
+    if filter_mask is None:
+        return i2 - i1
+    kept = getattr(filter_mask, "kept", None)
+    return len(blocks[0]) if blocks else (int(kept) if kept is not None else int(np.asarray(filter_mask).sum()))
 
 
 def decode_binner(spec, nthreads, hash_maps=None):
@@ -103,24 +108,21 @@ class TaskPartAggregation(TaskPart):
 
     def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
         # vaex/cpu.py:678-786
-        N = i2 - i1
-        if filter_mask is not None:  # the executor compacted the blocks with the filter (vaex/execution.py:516-522)
-            kept = getattr(filter_mask, "kept", None)
-            N = len(blocks[0]) if blocks else (int(kept) if kept is not None else int(np.asarray(filter_mask).sum()))
+        N = _rows(i1, i2, filter_mask, blocks)
         for block in blocks:
             assert len(block) == N, f"Oops, got a block of length {len(block)} while it is expected to be of length {N} (at {i1}-{i2}, filter={filter_mask is not None})"
         block_map = {expr: block for expr, block in zip(self.expressions, blocks)}
 
         def split(block):
             """-> (data, numpy-style mask or None); datetimes travel as integers (vaex/cpu.py:692-694)."""
-            if _is_device(block) or _hash.is_string_column(block):
+            if _hash.is_string_column(block):
                 return block, None  # string columns go to AggCount_string / AggNUnique_string as they are
-            if np.ma.isMaskedArray(block):
-                return np.ascontiguousarray(block.data), np.ma.getmaskarray(block)
-            block = np.asarray(block)
-            if block.dtype.kind in "mM":
-                block = block.view("uint64")
-            return block, None
+            data, mask = _lib.split_mask(block)
+            if not _lib.is_device(data):
+                data = np.asarray(data)
+                if data.dtype.kind in "mM":
+                    data = data.view("uint64")
+            return data, mask
 
         for binner in self.grid.binners:
             data, mask = split(block_map[binner.expression])
@@ -139,10 +141,7 @@ class TaskPartAggregation(TaskPart):
                 if not (selection is None or selection is False):
                     selection_mask = selection_masks[selection_index_global]
                     assert selection_mask is not None
-                    if not _is_device(selection_mask):
-                        selection_mask = np.asarray(selection_mask)
-                        if np.ma.isMaskedArray(selection_mask):  # vaex.utils.unmask_selection_mask
-                            selection_mask = selection_mask.data & ~np.ma.getmaskarray(selection_mask)
+                    selection_mask = _lib.unmask_selection(selection_mask)
                     # some aggregators make a distinction between missing value and no value (nunique): vaex/cpu.py:750-756
                     if hasattr(op, "set_selection_mask"):
                         op.set_selection_mask(thread_index, selection_mask)
@@ -203,49 +202,28 @@ class TaskPartAggregation(TaskPart):
         return encoded
 
 
-class TaskPartPercentile(TaskPartAggregation):
-    """percentile_approx / median_approx of one expression (vaex/dataframe.py:1632-1780): the count(*) pass over binby + [expression]
-    with edges (:1668-1672) on one device grid, then the finish on that grid (csrc/percentile.cu).  Only the percentiles are read
-    back; the count grid never leaves the device.  ``limit`` is the expression's (lb, ub) pair as the limits pre-pass returned it."""
-    snake_name = "percentile_approx"
+class TaskPartCountGrid(TaskPartAggregation):
+    """A count(*) pass with edges over `specs` on one device grid, then `finish(grid pointer, grid sizes, *args, ctx=...)` on that grid;
+    only the finish's answer is read back, the count grid never leaves the device.  Two analyses run through it:
+      * "percentile_approx": one expression of percentile_approx / median_approx (vaex/dataframe.py:1632-1780), binby + [expression]
+        (:1668-1672), finished by percentile.finish with args (the expression's (lb, ub) limit, percentage) (csrc/percentile.cu);
+      * "mutual_information": one combination of mutual_information (vaex/dataframe.py:685-819), combination + binby (:796-797),
+        finished by mutual_information.finish with args (the number of leading MI axes,) (csrc/mutinfo.cu)."""
 
-    def __init__(self, df, binners, aggregation_descriptions, dtypes, limit, percentage, nthreads=None):
-        super().__init__(df, binners, aggregation_descriptions, dtypes, nthreads=nthreads)
-        (desc, selections, ops, _), = self.aggregations
-        if len(ops) != 1 or desc.expressions:
-            raise ValueError("a percentile task part holds one count(*) aggregator with one selection")
-        self.limit = limit
-        self.percentage = percentage
-
-    def get_result(self):
-        from . import percentile as _pct
-        op = self.aggregations[0][2][0]
-        if op.device_dtype != np.int64:
-            raise RuntimeError("the percentile finish reads an int64 count grid")
-        ptr, _ = op.device_pointer(0)
-        return _pct.finish(ptr, self.grid.shapes, self.limit, self.percentage, op._ctx)
-
-
-class TaskPartMutualInformation(TaskPartAggregation):
-    """mutual_information of one combination (vaex/dataframe.py:685-819): the count(*) pass over combination + binby with edges
-    (:796-797) on one device grid, then the per-cell finish on that grid (csrc/mutinfo.cu).  Only one double per binby cell is read
-    back; the count grid never leaves the device.  ``dimension`` is the number of leading MI axes."""
-    snake_name = "mutual_information"
-
-    def __init__(self, df, binners, aggregation_descriptions, dtypes, dimension, nthreads=None):
-        super().__init__(df, binners, aggregation_descriptions, dtypes, nthreads=nthreads)
-        (desc, selections, ops, _), = self.aggregations
-        if len(ops) != 1 or desc.expressions:
-            raise ValueError("a mutual information task part holds one count(*) aggregator with one selection")
-        self.dimension = int(dimension)
+    def __init__(self, snake_name, specs, selection, dtypes, finish, args, nthreads=1):
+        desc = _agg.count("*", selection="selection" if selection else None, edges=True)
+        desc._prepare_types(dtypes)
+        super().__init__(None, [decode_binner(s, nthreads) for s in specs], [desc], dtypes, nthreads=nthreads)
+        self.snake_name = snake_name
+        self.finish = finish
+        self.args = tuple(args)
 
     def get_result(self):
-        from . import mutual_information as _mi
         op = self.aggregations[0][2][0]
         if op.device_dtype != np.int64:
-            raise RuntimeError("the mutual information finish reads an int64 count grid")
+            raise RuntimeError(f"the {self.snake_name} finish reads an int64 count grid")
         ptr, _ = op.device_pointer(0)
-        return _mi.finish(ptr, self.grid.shapes, self.dimension, op._ctx)
+        return self.finish(ptr, self.grid.shapes, *self.args, ctx=op._ctx)
 
 
 class RowLimitException(ValueError):
@@ -341,11 +319,9 @@ class TaskPartHashmapUniqueCreate(TaskPart):
 
 def _key_block(block):
     """a join key block -> (keys, mask or None): datetimes and timedeltas travel as int64 (vaex/join.py:192-193)"""
-    if _is_device(block):
+    block, mask = _lib.split_mask(block)
+    if _lib.is_device(block):
         return block, None
-    mask = None
-    if np.ma.isMaskedArray(block):
-        block, mask = np.ascontiguousarray(block.data), np.ma.getmaskarray(block)
     block = np.asarray(block)
     return (block.view(np.int64) if block.dtype.kind in "mM" else block), mask
 
@@ -393,7 +369,7 @@ class TaskPartLookup(TaskPart):
     def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
         keys, mask = _key_block(blocks[0])
         native = self.index._np_dtype()
-        if _is_device(keys) and np.dtype(keys.__cuda_array_interface__["typestr"]) != native:
+        if _lib.is_device(keys) and _lib.dtype_of(keys) != native:
             keys = _device_cast(keys, native, self._ctx)
         slot = self._ctx.slot(thread_index)
         out = self.lookup[i1:i2]
@@ -417,7 +393,7 @@ class TaskPartLookup(TaskPart):
 def _device_cast(keys, dtype, ctx):
     """a device key column of another dtype as `dtype`, where numpy would cast it safely (map_index refuses the rest)"""
     import torch
-    have = np.dtype(keys.__cuda_array_interface__["typestr"])
+    have = _lib.dtype_of(keys)
     if not np.can_cast(have, dtype, "safe"):
         raise TypeError(f"map_index: incompatible key dtype {have} (index dtype {dtype})")
     ctx.sync()  # a device expression's block is written on a slot's stream
@@ -456,17 +432,14 @@ class TaskPartStatistic(TaskPart):
 
     def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
         from . import statistic as _stat
-        N = i2 - i1
-        if filter_mask is not None:  # the executor compacted the blocks with the filter
-            kept = getattr(filter_mask, "kept", None)
-            N = len(blocks[0]) if blocks else (int(kept) if kept is not None else int(np.asarray(filter_mask).sum()))
+        N = _rows(i1, i2, filter_mask, blocks)
         nd = len(self.expressions)
         if not blocks and self.op.code != _stat.OP_ADD1.code:
             raise ValueError("Nothing to compute for OP %s" % self.op.code)
         for block in blocks[nd:]:
-            if _hash.is_string_column(block) or (not _is_device(block) and np.asarray(block).dtype.kind not in "biufmM"):
+            if _hash.is_string_column(block) or (not _lib.is_device(block) and np.asarray(block).dtype.kind not in "biufmM"):
                 raise NotImplementedError("the legacy statistic of a string or object column has no GPU path")
-        dtypes = [np.dtype(block.__cuda_array_interface__["typestr"]) if _is_device(block) else block.dtype for block in blocks]
+        dtypes = [_lib.dtype_of(block) for block in blocks]
         cls = _stat.compute_class(dtypes) if dtypes else _lib.F32
         sels = []
         for i, selection in enumerate(self.selections):
@@ -476,9 +449,7 @@ class TaskPartStatistic(TaskPart):
             mask = selection_masks[i]
             if mask is None:
                 raise ValueError("performing operation on selection while no selection present")
-            if not _is_device(mask):
-                mask = np.asarray(mask.data & ~np.ma.getmaskarray(mask)) if np.ma.isMaskedArray(mask) else np.asarray(mask)  # unmask_selection_mask
-            sels.append(mask)
+            sels.append(_lib.unmask_selection(mask))
         stat = self.stats.get(cls)
         if stat is None:
             stat = self.stats.setdefault(cls, _stat.Statistic(self.op.code, cls, self.shape, self.minima, self.maxima, self.edges,
@@ -548,14 +519,10 @@ class TaskPartMode(TaskPart):
         N = len(blocks[0])
         columns = []
         for block in blocks:
-            if _hash.is_string_column(block) or (not _is_device(block) and np.asarray(block).dtype.kind not in "biuf"):
+            if _hash.is_string_column(block) or (not _lib.is_device(block) and np.asarray(block).dtype.kind not in "biuf"):
                 raise NotImplementedError("mode of a string, object or datetime column has no GPU path")
-            columns.append(np.ma.getdata(block) if not _is_device(block) and np.ma.isMaskedArray(block) else block)
-        selection = None
-        if self.selection:
-            selection = selection_masks[0]
-            if not _is_device(selection) and np.ma.isMaskedArray(selection):  # unmask_selection_mask
-                selection = np.asarray(selection.data & ~np.ma.getmaskarray(selection))
+            columns.append(_lib.split_mask(block)[0])
+        selection = _lib.unmask_selection(selection_masks[0]) if self.selection else None
         self.histogram.bin(thread_index, columns, [], [selection], N, row_offset=i1)
         return i2 - i1
 
