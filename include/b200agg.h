@@ -416,6 +416,26 @@ int b200_take_strings(b200_ctx *ctx, int slot, const void *index, int index_isz,
                       const uint8_t *src_mask, int64_t src_len, int64_t *offsets_out, uint8_t *bytes_out, uint8_t *valid_out, int64_t capacity,
                       int64_t *size_needed, int32_t *missing_out);
 
+/* ---- argsort: df.sort (vaex/dataframe.py:4694-4745), whose pa.compute.sort_indices over the `by` columns runs here ------------
+ * perm_out (nrows int64, device memory) receives the stable permutation that sorts the rows by keys[0], then keys[1], ... with
+ * arrow's rules: -0.0 == +0.0, every NaN equal, NaN after every number and null after NaN in either direction, bool False < True,
+ * unsigned integers as unsigned, equal keys in row order also when descending.  Key data and masks are device memory, nrows items
+ * of the key's dtype (datetime / timedelta as B200_I64); mask (may be NULL): 1 = null; byteswap: 1 = non-native byte order;
+ * nat_is_null (B200_I64 only): INT64_MIN is null, as arrow converts a datetime column without a mask.  String keys are sorted
+ * through their ranks (an int64 key).  The scatter positions are 32-bit: at most B200_SORT_MAX_ROWS rows (B200_ERR_INVALID
+ * beyond, before anything is allocated).  Scratch from the context's block cache: 24 bytes per row plus the radix histograms.
+ * flags must be 0.  Runs on the slot's stream and returns when perm_out is written. */
+#define B200_SORT_MAX_KEYS 16
+#define B200_SORT_MAX_ROWS 4294967295ULL
+typedef struct {
+    const void *data;
+    int32_t dtype;       /* b200_dtype */
+    int32_t byteswap;
+    const uint8_t *mask; /* nullable, 1 = null */
+    int32_t descending;
+    int32_t nat_is_null;
+} b200_sort_key;
+int b200_argsort(b200_ctx *ctx, int slot, int nkeys, const b200_sort_key *keys, int64_t nrows, int64_t *perm_out, uint32_t flags);
 
 /* ---- host-chunk ingestion (SURVEY.md 8f row 2) ---------------------------------------------- */
 /* Page-lock a host column once (cudaHostRegister) so that the per-chunk H2D copies of b200_bin(HOST) run at PCIe rate and

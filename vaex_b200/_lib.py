@@ -17,7 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VAEX_B200_LIB") or os.path.join(_HERE, "libb200agg.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["api.cu", "binby.cu", "expr.cu", "fast.cu", "first.cu", "hashset.cu", "list.cu", "minmax.cu", "mutinfo.cu", "nunique.cu", "percentile.cu",
-           "ringcount.cu", "statistic.cu", "take.cu", "tilesort.cu"]
+           "ringcount.cu", "sort.cu", "statistic.cu", "take.cu", "tilesort.cu"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
@@ -43,6 +43,11 @@ class ExprOp(C.Structure):
 
 class ExprInput(C.Structure):
     _fields_ = [("data", C.c_void_p), ("dtype", C.c_int32), ("reserved", C.c_int32)]
+
+
+class SortKey(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("dtype", C.c_int32), ("byteswap", C.c_int32), ("mask", C.c_void_p), ("descending", C.c_int32),
+                ("nat_is_null", C.c_int32)]
 
 
 class AggInput(C.Structure):
@@ -131,6 +136,7 @@ def lib():
             "b200_compact": (i32, [vp, i32, vp, i32, P(vp), P(i32), i64, i32, P(vp), P(i64)]),
             "b200_take": (i32, [vp, i32, vp, i32, i64, i32, P(vp), P(i32), P(vp), i64, P(vp), P(vp), P(i32)]),
             "b200_take_strings": (i32, [vp, i32, vp, i32, i64, vp, i32, vp, vp, i64, vp, vp, vp, i64, P(i64), P(i32)]),
+            "b200_argsort": (i32, [vp, i32, i32, P(SortKey), i64, vp, u32]),
             "b200_set_dtype": (i32, [vp]),
             "b200_strset_create": (i32, [vp, i32, i64, P(vp)]),
             "b200_strset_update": (i32, [vp, i32, vp, vp, vp, i64, i32, vp, vp, i32]),

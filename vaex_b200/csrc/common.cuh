@@ -287,6 +287,9 @@ class CallFrame {
 };
 
 int slot_reserve(b200_ctx *ctx, Slot *s, size_t bytes);
+// the slot of a call that reads and writes device memory only and so needs no CallFrame (take.cu, sort.cu): checks the slot
+// (B200_ERR_INVALID naming `what`) and sets the device; the caller takes the slot's lock
+int device_slot(b200_ctx *ctx, int slot, const char *what, Slot **out);
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 

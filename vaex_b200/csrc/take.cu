@@ -120,9 +120,11 @@ int take_blocks(b200_ctx *ctx, unsigned long long threads) {
 
 bool index_size_ok(int isz) { return isz == 1 || isz == 2 || isz == 4 || isz == 8; }
 
-// the gathers read and write device memory only (the caller stages a host column once per join, not once per call), so they need
-// no call frame: the slot's stream, under the slot's lock, with the device set
-int take_slot(b200_ctx *ctx, int slot, const char *what, Slot **out) {
+} // namespace
+
+// the gathers (and the argsort of sort.cu) read and write device memory only (the caller stages a host column once, not once per
+// call), so they need no call frame: the slot's stream, under the slot's lock, with the device set
+int device_slot(b200_ctx *ctx, int slot, const char *what, Slot **out) {
     if (!ctx || slot < 0 || slot >= ctx->nslots) {
         set_error("%s: invalid slot %d", what, slot);
         return B200_ERR_INVALID;
@@ -132,7 +134,6 @@ int take_slot(b200_ctx *ctx, int slot, const char *what, Slot **out) {
     return B200_OK;
 }
 
-} // namespace
 } // namespace b200
 
 using namespace b200;
@@ -164,7 +165,7 @@ int b200_take(b200_ctx *ctx, int slot, const void *index, int index_isz, int64_t
     if (!n)
         return B200_OK;
     Slot *sl;
-    B200_CHECK(take_slot(ctx, slot, "b200_take", &sl));
+    B200_CHECK(device_slot(ctx, slot, "b200_take", &sl));
     std::lock_guard<std::mutex> g(sl->mu);
     DevBuf<unsigned> d_flags;
     B200_CHECK(d_flags.alloc(ctx, 4, "b200_take", sl->stream));
@@ -194,7 +195,7 @@ int b200_take_strings(b200_ctx *ctx, int slot, const void *index, int index_isz,
     *size_needed = 0;
     *missing_out = 0;
     Slot *sl;
-    B200_CHECK(take_slot(ctx, slot, "b200_take_strings", &sl));
+    B200_CHECK(device_slot(ctx, slot, "b200_take_strings", &sl));
     std::lock_guard<std::mutex> g(sl->mu);
     cudaStream_t st = sl->stream;
     // the byte range the source uses: offsets[0] .. offsets[src_len] (a sliced arrow array's offsets do not start at 0)

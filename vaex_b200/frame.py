@@ -40,11 +40,12 @@ class Frame:
     def __len__(self):
         return self.length
 
-    def _derive(self, columns, filter=None):
-        """a frame over `columns` with this frame's executor, categories, variables and, unless `filter` is given, its filter; the
-        filter is compiled again because a compiled expression is bound to its frame's column dict"""
-        return Frame(columns, executor=self.executor, categories=self.categories, filter=self._filter_expression if filter is None else filter,
-                     variables=self.variables)
+    def _derive(self, columns, filter=None, drop_filter=False):
+        """a frame over `columns` with this frame's executor, categories, variables and, unless `filter` is given or `drop_filter` is
+        true, its filter; the filter is compiled again because a compiled expression is bound to its frame's column dict"""
+        if filter is None and not drop_filter:
+            filter = self._filter_expression
+        return Frame(columns, executor=self.executor, categories=self.categories, filter=filter, variables=self.variables)
 
     def _with_columns(self, names):
         """this frame when every name is one of its columns, else a derived frame in which each missing name is a device-evaluated
@@ -583,6 +584,42 @@ class Frame:
         from . import join as _join
         return _join.join(self, other, on=on, left_on=left_on, right_on=right_on, lprefix=lprefix, rprefix=rprefix, lsuffix=lsuffix, rsuffix=rsuffix,
                           how=how, allow_duplication=allow_duplication, prime_growth=prime_growth, cardinality_other=cardinality_other, inplace=inplace)
+
+    # ---- sort and take: the argsort and the row gathers on the device (vaex_b200/sort.py) --------------------------------------
+    def take(self, indices, filtered=True, dropfilter=True):
+        """df.take (vaex/dataframe.py:4444-4481): a frame of the rows `indices` (a list, numpy array or device tensor of integers),
+        every real column gathered on the device (join's placement rule: device columns stay on the device, host ones come back to
+        the host, strings as arrow, masks kept) and the virtual columns kept virtual.  With `filtered` the indices count the rows that
+        pass this frame's filter; `dropfilter=False` keeps the filter over the taken rows.  An index outside [0, n) raises IndexError
+        (the reference's numpy indexing would wrap a negative one)."""
+        from . import sort as _sort
+        return self._taken(_sort.take_index(self, indices, filtered), dropfilter)
+
+    def sort(self, by, ascending=True):
+        """df.sort (vaex/dataframe.py:4694-4745): the filtered rows ordered by `by` (a name, an expression or a list of them) as
+        pa.compute.sort_indices orders them: stable, NaN after every number and null after NaN in either direction, strings bytewise.
+        `ascending` is a bool or a list of them (a key ascends only when its flag `is True`, as there).  The result has no filter;
+        a frame without rows that pass gives a copy of itself."""
+        from . import sort as _sort
+        by, ascending = _sort.normalize(by, ascending)
+        rows = _sort.sorted_rows(self, by, ascending)
+        if rows is None:
+            return self._derive(self.columns)
+        return self._taken(rows, True)
+
+    def _taken(self, index, dropfilter):
+        """a frame of the unfiltered rows `index`: real columns gathered, virtual ones over them, the filter dropped or kept"""
+        from . import expression as _expr
+        from . import join as _join
+        real = {k: v for k, v in self.columns.items() if not isinstance(v, _expr.DeviceExpression)}
+        out = self._derive(_join.gather(real, index, self.length, _lib.is_device), drop_filter=True)
+        for name, col in self.columns.items():
+            if isinstance(col, _expr.DeviceExpression):
+                out.add_virtual_column(name, col.expression)
+        out.columns = {name: out.columns[name] for name in self.columns}  # the column order of this frame
+        if not dropfilter and self._filter_expression is not None:
+            out = out.filter(self._filter_expression)
+        return out
 
     # ---- groupby ------------------------------------------------------------------------------------------------------
     def groupby(self, by, agg=None, sort=False, fused=True, combine=False):
