@@ -26,6 +26,35 @@ __device__ __forceinline__ void ldcs4<double>(const void *p, long long i, double
     out[2] = __longlong_as_double(((long long)b.y << 32) | b.x), out[3] = __longlong_as_double(((long long)b.w << 32) | b.z);
 }
 
+// ---- one element of an `isz`-byte (1, 2, 4 or 8) array as zero-extended raw bits -------------------------------------------------
+// ldcs1_raw is for the row columns above (read once, evict-first); load1_raw is a plain load for data that is read through an
+// index, read again or worth keeping in L2.
+__device__ __forceinline__ uint64_t load1_raw(const void *p, int isz, long long i) {
+    switch (isz) {
+    case 8: return static_cast<const unsigned long long *>(p)[i];
+    case 4: return static_cast<const unsigned *>(p)[i];
+    case 2: return static_cast<const unsigned short *>(p)[i];
+    default: return static_cast<const unsigned char *>(p)[i];
+    }
+}
+__device__ __forceinline__ uint64_t ldcs1_raw(const void *p, int isz, long long i) {
+    switch (isz) {
+    case 8: return __ldcs(static_cast<const unsigned long long *>(p) + i);
+    case 4: return __ldcs(static_cast<const unsigned *>(p) + i);
+    case 2: return __ldcs(static_cast<const unsigned short *>(p) + i);
+    default: return __ldcs(static_cast<const unsigned char *>(p) + i);
+    }
+}
+// the low `isz` bytes of v
+__host__ __device__ __forceinline__ void store1_raw(void *p, int isz, long long i, uint64_t v) {
+    switch (isz) {
+    case 8: static_cast<unsigned long long *>(p)[i] = v; break;
+    case 4: static_cast<unsigned *>(p)[i] = (unsigned)v; break;
+    case 2: static_cast<unsigned short *>(p)[i] = (unsigned short)v; break;
+    default: static_cast<unsigned char *>(p)[i] = (unsigned char)v; break;
+    }
+}
+
 __device__ __forceinline__ uint64_t bswap(uint64_t v, int isz) {
     switch (isz) {
     case 8: {

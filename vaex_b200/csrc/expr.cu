@@ -351,12 +351,7 @@ __global__ void __launch_bounds__(kCompactBlock) k_compact(const uint8_t *keep, 
         return;
     const unsigned long long pos = (unsigned long long)offsets[blockIdx.x] + warp_counts[warp] + __popc(m & ((1u << lane) - 1u));
     for (int c = 0; c < p.ncols; c++) {
-        switch (p.isz[c]) {
-        case 8: static_cast<unsigned long long *>(p.out[c])[pos] = static_cast<const unsigned long long *>(p.in[c])[i]; break;
-        case 4: static_cast<unsigned *>(p.out[c])[pos] = static_cast<const unsigned *>(p.in[c])[i]; break;
-        case 2: static_cast<unsigned short *>(p.out[c])[pos] = static_cast<const unsigned short *>(p.in[c])[i]; break;
-        default: static_cast<unsigned char *>(p.out[c])[pos] = static_cast<const unsigned char *>(p.in[c])[i]; break;
-        }
+        store1_raw(p.out[c], p.isz[c], pos, load1_raw(p.in[c], p.isz[c], i));
     }
 }
 

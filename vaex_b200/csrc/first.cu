@@ -99,15 +99,6 @@ __global__ void __launch_bounds__(kThreads) k_first_select(const __grid_constant
     }
 }
 
-__device__ __forceinline__ void store_raw(void *arr, int isz, unsigned long long i, uint64_t raw) {
-    switch (isz) {
-    case 8: static_cast<unsigned long long *>(arr)[i] = raw; break;
-    case 4: static_cast<unsigned *>(arr)[i] = (unsigned)raw; break;
-    case 2: static_cast<unsigned short *>(arr)[i] = (unsigned short)raw; break;
-    default: static_cast<unsigned char *>(arr)[i] = (unsigned char)raw; break;
-    }
-}
-
 template <bool VEC>
 __global__ void __launch_bounds__(kThreads) k_first_deposit(const __grid_constant__ FirstParams p) {
     const long long step = (long long)gridDim.x * kThreads * 4;
@@ -124,8 +115,8 @@ __global__ void __launch_bounds__(kThreads) k_first_deposit(const __grid_constan
                 continue;
             U128 cur = load128(p.state + 2 * idx[j]);
             if (cur.lo == c[j].kr.lo && cur.hi == c[j].kr.hi) { // exactly one row of the whole job matches
-                store_raw(p.grid, p.isz, idx[j], c[j].value_raw);
-                store_raw(p.order_grid, p.isz2, idx[j], c[j].order_raw);
+                store1_raw(p.grid, p.isz, idx[j], c[j].value_raw);
+                store1_raw(p.order_grid, p.isz2, idx[j], c[j].order_raw);
                 p.cell_masked[idx[j]] = 0;
             }
         }
@@ -143,18 +134,8 @@ __global__ void k_merge_first(unsigned long long *dstate, const unsigned long lo
             dstate[2 * i] = s.lo;
             dstate[2 * i + 1] = s.hi;
             dmask[i] = 0;
-            switch (isz) {
-            case 8: static_cast<unsigned long long *>(dgrid)[i] = static_cast<const unsigned long long *>(sgrid)[i]; break;
-            case 4: static_cast<unsigned *>(dgrid)[i] = static_cast<const unsigned *>(sgrid)[i]; break;
-            case 2: static_cast<unsigned short *>(dgrid)[i] = static_cast<const unsigned short *>(sgrid)[i]; break;
-            default: static_cast<unsigned char *>(dgrid)[i] = static_cast<const unsigned char *>(sgrid)[i]; break;
-            }
-            switch (isz2) {
-            case 8: static_cast<unsigned long long *>(dorder)[i] = static_cast<const unsigned long long *>(sorder)[i]; break;
-            case 4: static_cast<unsigned *>(dorder)[i] = static_cast<const unsigned *>(sorder)[i]; break;
-            case 2: static_cast<unsigned short *>(dorder)[i] = static_cast<const unsigned short *>(sorder)[i]; break;
-            default: static_cast<unsigned char *>(dorder)[i] = static_cast<const unsigned char *>(sorder)[i]; break;
-            }
+            store1_raw(dgrid, isz, i, load1_raw(sgrid, isz, i));
+            store1_raw(dorder, isz2, i, load1_raw(sorder, isz2, i));
         }
     }
 }

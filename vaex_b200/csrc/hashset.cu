@@ -90,15 +90,6 @@ constexpr unsigned long long kTagLowMask = (1ULL << 40) - 1;
 __host__ __device__ __forceinline__ unsigned long long index_bias(long long row) { return (unsigned long long)row ^ (1ull << 63); }
 __host__ __device__ __forceinline__ long long index_unbias(unsigned long long tag) { return (long long)(tag ^ (1ull << 63)); }
 
-__device__ __forceinline__ uint64_t load_raw1(const void *data, int isz, long long i) {
-    switch (isz) {
-    case 8: return __ldcs(static_cast<const unsigned long long *>(data) + i);
-    case 4: return __ldcs(static_cast<const unsigned *>(data) + i);
-    case 2: return __ldcs(static_cast<const unsigned short *>(data) + i);
-    default: return __ldcs(static_cast<const unsigned char *>(data) + i);
-    }
-}
-
 // insert (or touch) one key; returns false when the table is too full.  "Too full" is detected by PROBE LENGTH, not by a fill
 // counter: one shared counter bumped per new key serialises in the L2 (one update at a time to one address), while a
 // linear-probing table at load <= 0.5 practically never needs more than
@@ -145,7 +136,7 @@ __global__ void __launch_bounds__(256) k_set_insert(SetSlot *table, unsigned lon
         if (dead && (skip_keys & 2))
             return;
         const long long row = row0 + i;
-        uint64_t raw = load_raw1(keys, isz, row);
+        uint64_t raw = ldcs1_raw(keys, isz, row);
         bool isnull = from_keys ? (row == from_keys_null_index) : (masks && masks[row]);
         if (isnull) {
             if (!(skip_keys & 2)) { // bit 1: this range is being redone after a table growth — specials were already counted
@@ -193,7 +184,7 @@ __global__ void __launch_bounds__(256) k_set_count(const SetSlot *table, unsigne
                                                    int isz, const void *keys, const uint8_t *masks, const unsigned long long *weights, long long nrows) {
     unsigned long long n_sent = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
-        const uint64_t raw = load_raw1(keys, isz, i);
+        const uint64_t raw = ldcs1_raw(keys, isz, i);
         if ((masks && masks[i]) || raw_isnan(dtype, raw))
             continue; // NaN / null occurrences are counted by k_set_insert
         const unsigned long long w = weights ? weights[i] : 1ull;
@@ -332,15 +323,12 @@ __device__ __forceinline__ long long probe_lookup(const SetSlot *probe, unsigned
 __global__ void __launch_bounds__(256) k_set_map(const SetSlot *probe, unsigned long long mask, long long sentinel_ordinal, long long nan_ordinal, int dtype,
                                                  int isz, const void *keys, long long nrows, void *out, int out_isz) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
-        uint64_t raw = load_raw1(keys, isz, i);
+        uint64_t raw = ldcs1_raw(keys, isz, i);
         long long v = raw_isnan(dtype, raw) ? nan_ordinal : probe_lookup(probe, mask, sentinel_ordinal, key_canon(dtype, raw));
-        switch (out_isz) {
-        case 0: static_cast<unsigned char *>(out)[i] = v >= 0; break;
-        case 1: static_cast<signed char *>(out)[i] = (signed char)v; break;
-        case 2: static_cast<short *>(out)[i] = (short)v; break;
-        case 4: static_cast<int *>(out)[i] = (int)v; break;
-        default: static_cast<long long *>(out)[i] = v; break;
-        }
+        if (out_isz)
+            store1_raw(out, out_isz, i, (uint64_t)v);
+        else
+            static_cast<unsigned char *>(out)[i] = v >= 0;
     }
 }
 
@@ -364,7 +352,7 @@ __global__ void __launch_bounds__(256) k_set_combine(const __grid_constant__ Com
             if (p.masks[k] && p.masks[k][i]) {
                 o = p.null_ord[k];
             } else {
-                const uint64_t raw = load_raw1(p.keys[k], p.isz[k], i);
+                const uint64_t raw = ldcs1_raw(p.keys[k], p.isz[k], i);
                 o = raw_isnan(p.dtype[k], raw) ? p.nan_ord[k] : probe_lookup(p.probe[k], p.mask[k], p.sentinel[k], key_canon(p.dtype[k], raw));
             }
             missing |= o < 0;
@@ -379,7 +367,7 @@ __global__ void __launch_bounds__(256) k_set_values(const SetSlot *probe, unsign
                                                     long long null_ordinal, int dtype, int isz, int nmaps, const long long *offsets, const void *keys,
                                                     const uint8_t *masks, long long nrows, long long *out_values, short *out_map) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
-        uint64_t raw = load_raw1(keys, isz, i);
+        uint64_t raw = ldcs1_raw(keys, isz, i);
         if (masks && masks[i]) {
             out_values[i] = null_ordinal;
             out_map[i] = 0;
@@ -472,9 +460,8 @@ int set_finalize(b200_set *s) {
         return B200_ERR_UNSUPPORTED;
     }
     // one allocation: ckey | tag A | val A | tag B | val B | radix histograms | shard starts | special ordinals
-    const unsigned nblk = radix_blocks(E);
     const size_t en = (size_t)(E ? E : 1);
-    const size_t off_hist = 5 * en * 8, off_first = off_hist + align_up((size_t)256 * (nblk ? nblk : 1) * 4, 256), off_spec = off_first + align_up((size_t)s->nmaps * 8, 256);
+    const size_t off_hist = 5 * en * 8, off_first = off_hist + align_up(radix_scratch_bytes(E), 256), off_spec = off_first + align_up((size_t)s->nmaps * 8, 256);
     DevBuf<char> work;
     B200_CHECK(work.alloc(s->ctx, off_spec + 256, "set_finalize", st));
     unsigned long long *ckey = reinterpret_cast<unsigned long long *>(work.get()), *tagA = ckey + en, *valA = tagA + en, *tagB = valA + en, *valB = tagB + en;
@@ -514,26 +501,11 @@ int set_finalize(b200_set *s) {
         B200_CUDA(cudaMemcpyAsync(valA + n_table, xv, 8 * ne, cudaMemcpyHostToDevice, st));
     }
     unsigned long long *tin = tagA, *vin = valA, *tout = tagB, *vout = valB;
-    auto pass = [&](int shift, int from_val) -> int {
-        k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(tin, vin, E, shift, from_val, hist, nblk, radix_tiles(E));
-        k_scan_u32<<<1, 1024, 0, st>>>(hist, 256ull * nblk);
-        k_radix_scatter<<<nblk, kRadixThreads, 0, st>>>(tin, vin, tout, vout, E, shift, from_val, hist, nblk, radix_tiles(E));
-        B200_CUDA(cudaGetLastError());
-        std::swap(tin, tout);
-        std::swap(vin, vout);
-        return B200_OK;
-    };
-    if (E > 1) {
-        // tags are (call sequence << 40 | row): only the bytes that can differ are sorted on.  The NaN / null tags were moved just
-        // behind the largest row (see `special_tag`), so the row part stays below max_low.
-        const unsigned long long max_low = (unsigned long long)s->max_call_rows + 2, max_seq = (unsigned long long)(s->seq > 0 ? s->seq - 1 : 0);
-        for (int shift = 0; shift < 40 && (max_low >> shift); shift += 8)
-            B200_CHECK(pass(shift, 0));
-        for (int shift = 0; shift < 24 && (max_seq >> shift); shift += 8)
-            B200_CHECK(pass(40 + shift, 0));
-        for (int shift = 0; shift < 16 && ((unsigned)(s->nmaps - 1) >> shift); shift += 8)
-            B200_CHECK(pass(shift, 1));
-    }
+    // tags are (call sequence << 40 | row): only the bytes that can differ are sorted on, then (stable) the shard bytes of the
+    // payload.  The NaN / null tags were moved just behind the largest row (see `special_tag`), so the row part stays below max_low.
+    const unsigned long long max_low = (unsigned long long)s->max_call_rows + 2, max_seq = (unsigned long long)(s->seq > 0 ? s->seq - 1 : 0);
+    const unsigned tag_bytes = (radix_bytes_through(max_low) & 0x1fu) | (radix_bytes_through(max_seq) & 0x7u) << 5;
+    B200_CHECK(radix_sort(E, tag_bytes, radix_bytes_through((unsigned)(s->nmaps - 1)) & 0x3u, tin, vin, tout, vout, hist, st));
     // probe table + keys in ordinal order
     // (every reader of the previous probe table / key array holds s->mu or ran on a stream that has been synchronised since)
     B200_CHECK(b200_ctx_sync(s->ctx, -1));
@@ -669,7 +641,7 @@ __global__ void __launch_bounds__(256) k_index_log(unsigned long long *ctr, int 
         bool keep = false;
         unsigned long long canon = 0;
         if (i < nrows) {
-            const uint64_t raw = load_raw1(keys, isz, i);
+            const uint64_t raw = ldcs1_raw(keys, isz, i);
             if (masks && masks[i])
                 null_max = max(null_max, index_bias(start + i));
             else if (raw_isnan(dtype, raw))
@@ -752,7 +724,7 @@ __global__ void __launch_bounds__(256) k_index_map(const SetSlot *table, unsigne
     const IndexSpecials sp = index_specials(ctr);
     bool unk = false;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
-        const uint64_t raw = load_raw1(keys, isz, i);
+        const uint64_t raw = ldcs1_raw(keys, isz, i);
         long long v;
         if (raw_isnan(dtype, raw)) {
             v = sp.nan_row;
@@ -783,12 +755,7 @@ __global__ void __launch_bounds__(256) k_index_map(const SetSlot *table, unsigne
             }
             unk |= !found;
         }
-        switch (out_isz) {
-        case 1: static_cast<signed char *>(out)[i] = (signed char)v; break;
-        case 2: static_cast<short *>(out)[i] = (short)v; break;
-        case 4: static_cast<int *>(out)[i] = (int)v; break;
-        default: static_cast<long long *>(out)[i] = v; break;
-        }
+        store1_raw(out, out_isz, i, (uint64_t)v);
     }
     if (unk)
         *unknown = 1;
@@ -797,7 +764,7 @@ __global__ void __launch_bounds__(256) k_index_map(const SetSlot *table, unsigne
 // the overflow range of a left row's key: [begin + 1, end) of its slot (the primary row is excluded); NaN and masked rows have none
 __device__ __forceinline__ uint2 index_overflow(const SetSlot *table, unsigned long long mask, const uint2 *seg, int dtype, int isz, const void *keys,
                                                 const uint8_t *masks, long long i) {
-    const uint64_t raw = load_raw1(keys, isz, i);
+    const uint64_t raw = ldcs1_raw(keys, isz, i);
     if ((masks && masks[i]) || raw_isnan(dtype, raw))
         return make_uint2(0, 0);
     const unsigned long long slot = index_slot(table, mask, key_canon(dtype, raw));
@@ -913,29 +880,16 @@ int index_sort(b200_set *s, cudaStream_t st) {
     B200_CUDA(cudaMemsetAsync(s->idx_seg, 0, nslots * sizeof(uint2), st));
     B200_CHECK(s->idx_rows.alloc(s->ctx, (E ? E : 1) * 8, "index_hash ranges"));
     if (E) {
-        const unsigned nblk = radix_blocks(E);
         const size_t off_hist = 4 * E * 8;
         DevBuf<char> work;
-        B200_CHECK(work.alloc(s->ctx, off_hist + (size_t)256 * nblk * 4, "index_hash sort", st));
+        B200_CHECK(work.alloc(s->ctx, off_hist + radix_scratch_bytes(E), "index_hash sort", st));
         unsigned long long *tin = reinterpret_cast<unsigned long long *>(work.get()), *vin = tin + E, *tout = vin + E, *vout = tout + E;
         unsigned *hist = reinterpret_cast<unsigned *>(work + off_hist);
         k_index_sort_keys<<<nblocks(E), 256, 0, st>>>(s->table, s->cap - 1, s->log_key, s->log_row, E, s->row_min, tin, vin);
         B200_CUDA(cudaGetLastError());
-        auto pass = [&](int shift, int from_val) -> int {
-            k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(tin, vin, E, shift, from_val, hist, nblk, radix_tiles(E));
-            k_scan_u32<<<1, 1024, 0, st>>>(hist, 256ull * nblk);
-            k_radix_scatter<<<nblk, kRadixThreads, 0, st>>>(tin, vin, tout, vout, E, shift, from_val, hist, nblk, radix_tiles(E));
-            B200_CUDA(cudaGetLastError());
-            std::swap(tin, tout);
-            std::swap(vin, vout);
-            return B200_OK;
-        };
         // LSD: the row bytes that vary, then (stable) the slot bytes
         const unsigned long long row_span = (unsigned long long)(s->row_max - s->row_min);
-        for (int shift = 0; shift < 64 && (row_span >> shift); shift += 8)
-            B200_CHECK(pass(shift, 0));
-        for (int shift = 0; shift < 32 && (s->cap >> shift); shift += 8)
-            B200_CHECK(pass(shift, 1));
+        B200_CHECK(radix_sort(E, radix_bytes_through(row_span), radix_bytes_through(s->cap) & 0xfu, tin, vin, tout, vout, hist, st));
         k_index_segments<<<nblocks(E), 256, 0, st>>>(tin, vin, E, s->row_min, s->idx_rows, s->idx_seg);
         B200_CUDA(cudaGetLastError());
         B200_CUDA(cudaStreamSynchronize(st));
@@ -1396,12 +1350,7 @@ int b200_set_key_array(b200_set *s, void *out) {
             else
                 bits = ~0ull;
         }
-        switch (isz) {
-        case 8: static_cast<uint64_t *>(out)[i] = bits; break;
-        case 4: static_cast<uint32_t *>(out)[i] = (uint32_t)bits; break;
-        case 2: static_cast<uint16_t *>(out)[i] = (uint16_t)bits; break;
-        default: static_cast<uint8_t *>(out)[i] = (uint8_t)bits; break;
-        }
+        store1_raw(out, isz, i, bits);
     }
     return B200_OK;
 }

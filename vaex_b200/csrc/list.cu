@@ -105,12 +105,7 @@ __global__ void k_list_values(const unsigned long long *keys, const unsigned lon
             v = dtype == B200_F64 ? 0x7ff8000000000000ull : 0x7fc00000ull;
         else if (cat == 2)
             v = 0; // the reference leaves these slots unwritten
-        switch (isz) {
-        case 8: static_cast<unsigned long long *>(out)[i] = v; break;
-        case 4: static_cast<unsigned *>(out)[i] = (unsigned)v; break;
-        case 2: static_cast<unsigned short *>(out)[i] = (unsigned short)v; break;
-        default: static_cast<unsigned char *>(out)[i] = (unsigned char)v; break;
-        }
+        store1_raw(out, isz, i, v);
     }
 }
 
@@ -289,21 +284,13 @@ static int list_sort_count(b200_agg *a, cudaStream_t st, unsigned long long maxk
             set_error("AggList: more than 2^32 rows are not supported");
             return B200_ERR_UNSUPPORTED;
         }
-        const unsigned nblk = radix_blocks(n), tiles = radix_tiles(n);
         DevBuf<unsigned long long> kb, vb;
         DevBuf<unsigned> hist;
         B200_CHECK(kb.alloc(a->ctx, n * 8, "b200_agg_list_finish", st));
         B200_CHECK(vb.alloc(a->ctx, n * 8, "b200_agg_list_finish", st));
-        B200_CHECK(hist.alloc(a->ctx, (size_t)256 * nblk * 4, "b200_agg_list_finish", st));
+        B200_CHECK(hist.alloc(a->ctx, radix_scratch_bytes(n), "b200_agg_list_finish", st));
         unsigned long long *kin = a->list_keys, *vin = a->list_vals, *kout = kb, *vout = vb;
-        for (int shift = 0; shift < 64 && (maxkey >> shift); shift += 8) {
-            k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(kin, vin, n, shift, 0, hist, nblk, tiles);
-            k_scan_u32<<<1, 1024, 0, st>>>(hist, 256ull * nblk);
-            k_radix_scatter<<<nblk, kRadixThreads, 0, st>>>(kin, vin, kout, vout, n, shift, 0, hist, nblk, tiles);
-            B200_CUDA(cudaGetLastError());
-            std::swap(kin, kout);
-            std::swap(vin, vout);
-        }
+        B200_CHECK(radix_sort(n, radix_bytes_through(maxkey), 0, kin, vin, kout, vout, hist, st));
         if (kin != a->list_keys) { // an odd number of passes: the sorted records sit in the scratch arrays, which have n entries
             B200_CUDA(cudaMemcpyAsync(a->list_keys, kin, n * 8, cudaMemcpyDeviceToDevice, st));
             B200_CUDA(cudaMemcpyAsync(a->list_vals, vin, n * 8, cudaMemcpyDeviceToDevice, st));

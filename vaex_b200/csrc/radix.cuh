@@ -1,14 +1,17 @@
-// radix.cuh — stable LSD radix sort passes over (64-bit key, 64-bit payload) pairs, shared by the ordered_set finalisation
-// (hashset.cu) and the list aggregator (list.cu).
+// radix.cuh — stable LSD radix sort of (64-bit key, 64-bit payload) pairs, one driver (radix_sort) for every device sort: the
+// ordered_set finalisation and the index_hash row ranges (hashset.cu), the argsort (sort.cu) and the list aggregator (list.cu).
 #pragma once
+#include <algorithm>
+
 #include "common.cuh"
+#include "scan.cuh"
 
 namespace b200 {
 
 // ---- LSD radix sort of (64-bit sort key, 64-bit payload) pairs, 8 bits per pass, stable --------------------------------------
 // Replaces round 1's bitonic network (210 launches for 2^20 entries) + a 24 MB download + a host loop.  One pass = per-block digit
 // histograms (digit-major), one exclusive scan over the 256 x nblocks matrix, a stable scatter.  `from_val`: the digit comes from
-// the payload's upper word (the shard) instead of the key.
+// the payload's upper word instead of the key.
 constexpr int kRadixThreads = 256;
 
 // A block sorts a TILE of `tiles` consecutive sub-tiles of 256 pairs (in order, so the pass stays stable); the tile size grows
@@ -91,6 +94,40 @@ static __global__ void __launch_bounds__(kRadixThreads) k_radix_scatter(const un
         __syncthreads();
         run[threadIdx.x] += total;
     }
+}
+
+// the histogram scratch radix_sort needs for n pairs
+static inline size_t radix_scratch_bytes(unsigned long long n) { return (size_t)256 * 4 * std::max(radix_blocks(n), 1u); }
+
+// every byte of x through its highest non-zero one: the byte set that orders values in [0, x]
+static inline unsigned radix_bytes_through(unsigned long long x) {
+    unsigned bytes = 0;
+    for (int b = 0; b < 8 && (x >> (8 * b)); b++)
+        bytes |= 1u << b;
+    return bytes;
+}
+
+// Enqueues on `st` a stable LSD sort of the n pairs (key[i], val[i]): one pass for every bit b of key_bytes, on key byte b, least
+// significant first, then one for every bit b (0-3) of val_bytes, on byte b of val >> 32.  Each pass moves the pairs between
+// (key, val) and (key_alt, val_alt); on return key / val point at the sorted pairs and key_alt / val_alt at the other two arrays.
+// hist holds radix_scratch_bytes(n).  Nothing is allocated and nothing is synchronised: the caller orders what follows on `st`.
+static inline int radix_sort(unsigned long long n, unsigned key_bytes, unsigned val_bytes, unsigned long long *&key, unsigned long long *&val,
+                             unsigned long long *&key_alt, unsigned long long *&val_alt, unsigned *hist, cudaStream_t st) {
+    if (n < 2)
+        return B200_OK;
+    const unsigned nblk = radix_blocks(n), tiles = radix_tiles(n);
+    for (int pass = 0; pass < 12; pass++) {
+        const int from_val = pass >= 8, b = from_val ? pass - 8 : pass;
+        if (!(((from_val ? val_bytes : key_bytes) >> b) & 1u))
+            continue;
+        k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(key, val, n, 8 * b, from_val, hist, nblk, tiles);
+        k_scan_u32<<<1, 1024, 0, st>>>(hist, 256ull * nblk);
+        k_radix_scatter<<<nblk, kRadixThreads, 0, st>>>(key, val, key_alt, val_alt, n, 8 * b, from_val, hist, nblk, tiles);
+        B200_CUDA(cudaGetLastError());
+        std::swap(key, key_alt);
+        std::swap(val, val_alt);
+    }
+    return B200_OK;
 }
 
 

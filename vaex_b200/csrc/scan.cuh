@@ -1,4 +1,4 @@
-// scan.cuh — exclusive scans in place: u32 counters in one CTA (shared by the radix sort of hashset.cu and the filter compaction
+// scan.cuh — exclusive scans in place: u32 counters in one CTA (shared by the radix sort of radix.cuh and the filter compaction
 // of expr.cu: n is a few million at most), and int64 values of any length over many CTAs (list.cu).
 #pragma once
 #include "common.cuh"

@@ -15,8 +15,8 @@
 // a radix pass reads 8 (histogram) + 16 bytes and writes 16 per row.  The scatter's positions are 32-bit: n < 2^32.
 #include <algorithm>
 
+#include "device_utils.cuh"
 #include "radix.cuh"
-#include "scan.cuh"
 
 namespace b200 {
 namespace {
@@ -40,31 +40,14 @@ struct EncodeParams {
 
 __host__ __device__ inline int value_bits(int dtype) { return dtype == B200_BOOL ? 1 : 8 * dtype_size(dtype); }
 
-__device__ __forceinline__ unsigned long long load_raw(const void *d, int isz, long long r, int bswap) {
-    switch (isz) {
-    case 1: return static_cast<const uint8_t *>(d)[r];
-    case 2: {
-        const unsigned short v = static_cast<const unsigned short *>(d)[r];
-        return bswap ? (unsigned short)((v >> 8) | (v << 8)) : v;
-    }
-    case 4: {
-        const unsigned v = static_cast<const unsigned *>(d)[r];
-        return bswap ? __byte_perm(v, 0, 0x0123) : v;
-    }
-    default: {
-        const unsigned long long v = static_cast<const unsigned long long *>(d)[r];
-        if (!bswap)
-            return v;
-        return ((unsigned long long)__byte_perm((unsigned)v, 0, 0x0123) << 32) | __byte_perm((unsigned)(v >> 32), 0, 0x0123);
-    }
-    }
-}
-
 // the class (0 value, 1 NaN, 2 null) and the order-preserving value bits of key k at row r
 __device__ __forceinline__ int encode_key(const EncodeParams &p, int k, long long r, unsigned long long *value) {
     const int dt = p.dtype[k], bits = value_bits(dt);
     const unsigned long long full = bits == 64 ? ~0ull : (1ull << bits) - 1ull, top = 1ull << (bits - 1);
-    unsigned long long v = load_raw(p.data[k], dtype_size(dt), r, p.byteswap[k]);
+    const int isz = dtype_size(dt);
+    unsigned long long v = load1_raw(p.data[k], isz, r);
+    if (p.byteswap[k])
+        v = bswap(v, isz);
     int cls = p.mask[k] && p.mask[k][r] ? 2 : 0;
     switch (dt) {
     case B200_F64:
@@ -196,9 +179,8 @@ int b200_argsort(b200_ctx *ctx, int slot, int nkeys, const b200_sort_key *keys, 
     std::lock_guard<std::mutex> g(sl->mu);
     cudaStream_t st = sl->stream;
     const unsigned long long n = (unsigned long long)nrows;
-    const unsigned nblk = radix_blocks(n), tiles = radix_tiles(n);
     // scratch: word A | word B | payload B (payload A is perm_out) | radix histograms | AND / OR
-    const size_t off_hist = 3 * n * 8, off_andor = off_hist + align_up((size_t)256 * nblk * 4, 256);
+    const size_t off_hist = 3 * n * 8, off_andor = off_hist + align_up(radix_scratch_bytes(n), 256);
     DevBuf<char> work;
     B200_CHECK(work.alloc(ctx, off_andor + 16, "b200_argsort", st));
     unsigned long long *win = reinterpret_cast<unsigned long long *>(work.get()), *wout = win + n;
@@ -219,17 +201,12 @@ int b200_argsort(b200_ctx *ctx, int slot, int nkeys, const b200_sort_key *keys, 
         unsigned long long h[2];
         B200_CUDA(cudaMemcpyAsync(h, andor, 16, cudaMemcpyDeviceToHost, st));
         B200_CUDA(cudaStreamSynchronize(st));
+        // a byte every row shares orders nothing
         const unsigned long long varying = h[0] ^ h[1];
-        for (int shift = 0; shift < 64; shift += 8) {
-            if (!((varying >> shift) & 255u))
-                continue; // a byte every row shares orders nothing
-            k_radix_hist<<<nblk, kRadixThreads, 0, st>>>(win, pin, n, shift, 0, hist, nblk, tiles);
-            k_scan_u32<<<1, 1024, 0, st>>>(hist, 256ull * nblk);
-            k_radix_scatter<<<nblk, kRadixThreads, 0, st>>>(win, pin, wout, pout, n, shift, 0, hist, nblk, tiles);
-            B200_CUDA(cudaGetLastError());
-            std::swap(win, wout);
-            std::swap(pin, pout);
-        }
+        unsigned bytes = 0;
+        for (int b = 0; b < 8; b++)
+            bytes |= ((varying >> (8 * b)) & 255u) ? 1u << b : 0u;
+        B200_CHECK(radix_sort(n, bytes, 0, win, pin, wout, pout, hist, st));
     }
     if (pin != reinterpret_cast<unsigned long long *>(perm_out))
         B200_CUDA(cudaMemcpyAsync(perm_out, pin, n * 8, cudaMemcpyDeviceToDevice, st));

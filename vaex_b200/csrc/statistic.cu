@@ -120,17 +120,6 @@ __device__ __forceinline__ int stat_bin(const StatParams &p, int d, T v) {
     return min(b, size - 1);
 }
 
-__device__ __forceinline__ uint64_t load_raw(const StatCol &c, long long i) {
-    uint64_t r;
-    switch (c.isz) {
-    case 8: r = __ldcs(static_cast<const unsigned long long *>(c.data) + i); break;
-    case 4: r = __ldcs(static_cast<const unsigned *>(c.data) + i); break;
-    case 2: r = __ldcs(static_cast<const unsigned short *>(c.data) + i); break;
-    default: r = __ldcs(static_cast<const unsigned char *>(c.data) + i); break;
-    }
-    return r;
-}
-
 template <typename T>
 __device__ __forceinline__ double col_value(const StatCol &c, uint64_t r) {
     return (double)raw_class_value<T>(c.dt, c.swap ? bswap(r, c.isz) : r);
@@ -219,7 +208,7 @@ __device__ __forceinline__ void apply_atomic(const StatParams &p, unsigned long 
         }
     } else if constexpr (OP == B200_STAT_COV) {
         const int n = NT ? NT : p.nw, P = cov_pairs(n), nc = p.nc;
-        auto val = [&](int i) { return NT ? wv[i] : col_value<T>(p.w[i], load_raw(p.w[i], row)); };
+        auto val = [&](int i) { return NT ? wv[i] : col_value<T>(p.w[i], ldcs1_raw(p.w[i].data, p.w[i].isz, row)); };
         for (int i = 0; i < n; i++) {
             const double x = val(i);
             if (isnan_d(x))

@@ -11,6 +11,7 @@
 // is read at L2 rate; beyond that each 1-8 byte item costs a 32-byte HBM sector.
 #include <algorithm>
 
+#include "device_utils.cuh"
 #include "scan.cuh"
 #include "strings.cuh"
 
@@ -38,15 +39,6 @@ __device__ __forceinline__ long long load_index(const void *index, int isz, long
     }
 }
 
-__device__ __forceinline__ void copy_item(const void *src, void *dst, int isz, long long from, long long to, bool zero) {
-    switch (isz) {
-    case 1: static_cast<uint8_t *>(dst)[to] = zero ? 0 : static_cast<const uint8_t *>(src)[from]; break;
-    case 2: static_cast<uint16_t *>(dst)[to] = zero ? 0 : static_cast<const uint16_t *>(src)[from]; break;
-    case 4: static_cast<uint32_t *>(dst)[to] = zero ? 0 : static_cast<const uint32_t *>(src)[from]; break;
-    default: static_cast<unsigned long long *>(dst)[to] = zero ? 0 : static_cast<const unsigned long long *>(src)[from]; break;
-    }
-}
-
 // one thread per output row (grid-stride); the per-thread flag bits are OR-ed over the warp and written with one atomic per warp
 __global__ void __launch_bounds__(256) k_take(const void *__restrict__ index, int index_isz, long long n, long long src_len, TakeParams p,
                                               unsigned *flags) {
@@ -58,7 +50,7 @@ __global__ void __launch_bounds__(256) k_take(const void *__restrict__ index, in
         const bool none = idx < 0 || bad;
         for (int c = 0; c < p.ncols; c++) {
             const bool missing = none || (p.src_mask[c] && p.src_mask[c][idx]);
-            copy_item(p.src[c], p.dst[c], p.isz[c], idx, i, none);
+            store1_raw(p.dst[c], p.isz[c], i, none ? 0 : load1_raw(p.src[c], p.isz[c], idx)); // a miss's index may be out of range
             if (p.dst_valid[c])
                 p.dst_valid[c][i] = missing ? 0 : 1;
             bits |= missing ? 1u << c : 0u;
