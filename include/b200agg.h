@@ -70,10 +70,25 @@ typedef enum {
 typedef enum {
     B200_BINNER_SCALAR = 0,  /* BinnerScalar_<T>  */
     B200_BINNER_ORDINAL = 1, /* BinnerOrdinal_<T> */
-    B200_BINNER_HASH = 2     /* ordinal binner fed by a fused ordered_set probe: the reference's
+    B200_BINNER_HASH = 2,    /* ordinal binner fed by a fused ordered_set probe: the reference's
                                 `_ordinal_values(key, set)` expression (vaex/functions.py:2454-2463) +
                                 BinnerOrdinal (vaex/groupby.py:303-317) without materialising the codes */
+    B200_BINNER_TIME = 3     /* BinnerTime (vaex/groupby.py:63-135): the reference's `(t.astype('M8[R]') - begin).astype('int') // every`
+                                fed to BinnerOrdinal, with the calendar period computed in the binning kernel.  `data` holds the raw
+                                int64 ticks of a datetime64 column (dtype B200_I64); `reserved` = unit | resolution << 8, both
+                                b200_time_unit codes; `min_value` = begin, the first period in the resolution; `ordinal_count` = N
+                                >= 1 bins; `bins` = every >= 1; allow_other and invert must be 0.  A row's period is numpy's
+                                astype('M8[R]') (floor towards -inf, weeks counted from Thursday 1970-01-01, months and years from
+                                the proleptic Gregorian calendar, multiplication that wraps for a finer resolution); its bin is
+                                floor((period - begin) / every).  NaT (INT64_MIN), masked rows and bins outside [0, N) land in
+                                cell N, like every other BinnerOrdinal; cells are N + 2.  byteswap: the ticks are swapped first. */
 } b200_binner_kind;
+
+/* numpy datetime64 units, coarsest first (B200_BINNER_TIME) */
+typedef enum {
+    B200_TIME_Y = 0, B200_TIME_M, B200_TIME_W, B200_TIME_D, B200_TIME_h, B200_TIME_m, B200_TIME_s, B200_TIME_ms, B200_TIME_us,
+    B200_TIME_ns, B200_TIME_NUNITS
+} b200_time_unit;
 
 typedef enum {
     B200_AGG_COUNT = 0, B200_AGG_SUM, B200_AGG_SUM_MOMENT, B200_AGG_MIN, B200_AGG_MAX,
@@ -114,10 +129,10 @@ typedef struct {
     int32_t byteswap;    /* 1 = the `_non_native` class variant (FlipEndian) */
     int32_t allow_other; /* ordinal */
     int32_t invert;      /* ordinal */
-    int32_t reserved;
+    int32_t reserved;    /* TIME: unit | resolution << 8 */
     double vmin, vmax;   /* scalar */
-    uint64_t bins;       /* scalar */
-    int64_t ordinal_count, min_value; /* ordinal (for HASH: ordinal_count = number of codes, min_value 0) */
+    uint64_t bins;       /* scalar; TIME: every */
+    int64_t ordinal_count, min_value; /* ordinal (for HASH: ordinal_count = number of codes, min_value 0; TIME: N, begin) */
     const b200_set *set; /* HASH only */
     const void *data;
     const uint8_t *mask; /* nullable */

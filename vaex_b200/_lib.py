@@ -24,7 +24,9 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 DTYPES = ["float64", "float32", "int64", "int32", "int16", "int8", "uint64", "uint32", "uint16", "uint8", "bool"]
 DTYPE_CODE = {n: i for i, n in enumerate(DTYPES)}
 F64, F32, I64, I32, I16, I8, U64, U32, U16, U8, BOOL = range(11)
-BINNER_SCALAR, BINNER_ORDINAL, BINNER_HASH = 0, 1, 2
+BINNER_SCALAR, BINNER_ORDINAL, BINNER_HASH, BINNER_TIME = 0, 1, 2, 3
+# numpy datetime64 units in b200_time_unit order (include/b200agg.h)
+TIME_UNITS = ["Y", "M", "W", "D", "h", "m", "s", "ms", "us", "ns"]
 AGG_COUNT, AGG_SUM, AGG_SUM_MOMENT, AGG_MIN, AGG_MAX, AGG_FIRST, AGG_LAST, AGG_NUNIQUE, AGG_LIST, AGG_LIST_STRING = range(10)
 MEM_HOST, MEM_DEVICE, MEM_MIXED = 0, 1, 2
 FLAG_ASYNC_HOST = 1
@@ -317,6 +319,33 @@ def dtype_of(col):
     if is_device(col):
         return np.dtype(col.__cuda_array_interface__["typestr"])
     return col.dtype if np.ma.isMaskedArray(col) else np.asarray(col).dtype
+
+
+class _Int64View:
+    """a device datetime64 / timedelta64 column seen as its int64 ticks: the same memory and byte order, sliceable like a column"""
+
+    def __init__(self, col, offset=0, length=None):
+        cai = col.__cuda_array_interface__
+        self._col, self._offset = col, offset
+        self._length = cai["shape"][0] if length is None else length
+        self.dtype = np.dtype("int64").newbyteorder(np.dtype(cai["typestr"]).byteorder)
+        self.__cuda_array_interface__ = {"shape": (self._length,), "typestr": self.dtype.str, "data": (cai["data"][0] + 8 * offset, False),
+                                         "version": 3, "strides": None}
+
+    def __len__(self):
+        return self._length
+
+    def __getitem__(self, s):
+        i1, i2, _ = s.indices(self._length)
+        return _Int64View(self._col, self._offset + i1, max(i2 - i1, 0))
+
+
+def int64_view(block):
+    """a datetime64 / timedelta64 block as its signed int64 ticks (numpy's astype(int) reading), without a copy"""
+    if is_device(block):
+        return _Int64View(block)
+    block = np.asarray(block)
+    return block.view(np.dtype(np.int64).newbyteorder(block.dtype.byteorder))
 
 
 def split_mask(block):

@@ -979,6 +979,20 @@ int b200_bin(b200_ctx *ctx, int slot, const b200_binner *binners, int nbinners, 
             } else {
                 d.byteswap = b.byteswap != 0; // the ordinal FlipEndian quirk flips the int64 difference, any itemsize
             }
+        } else if (b.kind == B200_BINNER_TIME) {
+            const int unit = b.reserved & 0xff, res = (b.reserved >> 8) & 0xff;
+            if (b.dtype != B200_I64 || (b.reserved >> 16) || unit >= B200_TIME_NUNITS || res >= B200_TIME_NUNITS || b.ordinal_count < 1 ||
+                b.bins < 1 || b.bins > (uint64_t)INT64_MAX || b.allow_other || b.invert) {
+                set_error("b200_bin: binner %d: time binner needs int64 ticks, unit and resolution codes below %d, N >= 1, 1 <= every < 2^63 "
+                          "and neither allow_other nor invert (dtype %d, reserved %#x, N %lld, every %llu)",
+                          i, B200_TIME_NUNITS, b.dtype, b.reserved, (long long)b.ordinal_count, (unsigned long long)b.bins);
+                return B200_ERR_INVALID;
+            }
+            d.time = time_steps(unit, res);
+            d.every = make_divisor(b.bins);
+            d.ordinal_count = b.ordinal_count;
+            d.min_value = b.min_value;
+            shape = (unsigned long long)b.ordinal_count + 2;
         } else {
             set_error("b200_bin: binner %d: unknown kind %d", i, b.kind);
             return B200_ERR_INVALID;

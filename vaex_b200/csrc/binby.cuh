@@ -6,6 +6,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "device_utils.cuh"
 
 namespace b200 {
 
@@ -30,6 +31,9 @@ struct DevBinner {
     long long nan_ordinal;      // -1 when the set saw no NaN
     long long null_ordinal;     // -1 when the set saw no null (masked rows then fall into the null cell)
     long long sentinel_ordinal; // ordinal of the key whose pattern equals SET_EMPTY, -1 if absent
+    // B200_BINNER_TIME (time_period in device_utils.cuh): begin = min_value, N = ordinal_count
+    TimeSteps time;
+    Divisor every;
 };
 
 struct DevAgg {

@@ -46,6 +46,12 @@ __device__ __forceinline__ void binby_indices(const DevBinner *__restrict__ binn
                 long long value = ordinal_value(b.dtype, r[j], b.min_value, b.byteswap != 0);
                 idx[j] += ordinal_index(value, m[j] == 1, b.ordinal_count, b.allow_other != 0, b.invert != 0) * b.stride;
             }
+        } else if (b.kind == B200_BINNER_TIME) {
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const long long t = (long long)(b.byteswap ? bswap(r[j], 8) : r[j]);
+                idx[j] += ordinal_index(time_bin(t, m[j] == 1, b.time, b.min_value, b.every), false, b.ordinal_count, false, false) * b.stride;
+            }
         } else { // B200_BINNER_HASH: HashMapUnique.map (vaex/hash.py:193-214) + BinnerOrdinal
 #pragma unroll
             for (int j = 0; j < 4; j++) {

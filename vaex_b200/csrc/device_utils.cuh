@@ -234,6 +234,108 @@ __device__ __forceinline__ unsigned long long ordinal_index(long long value, boo
     return (unsigned long long)(invert ? n - 1 - value : value);
 }
 
+// ---- BinnerTime: numpy's datetime64 astype('M8[R]') on raw int64 ticks (B200_BINNER_TIME) ---------------------------------------
+// floor(n / d) for a divisor d >= 1 known only at run time, without a 64-bit division per row: for 0 <= u < 2^63,
+// floor(u / d) = umulhi(u, magic) >> shift with l = ceil(log2 d), magic = ceil(2^(63 + l) / d) (< 2^64), shift = l - 1 (the error
+// of magic / 2^(63 + l) against 1 / d is below 2^-l / 2^63, too small to carry u / d over the next integer).  magic = 0: d = 1.
+struct Divisor {
+    unsigned long long magic;
+    int shift;
+};
+inline Divisor make_divisor(unsigned long long d) {
+    Divisor v{0, 0};
+    if (d <= 1)
+        return v;
+    int l = 0;
+    while (l < 64 && (1ull << l) < d)
+        l++;
+    const unsigned __int128 num = (unsigned __int128)1 << (63 + l);
+    v.magic = (unsigned long long)((num + d - 1) / d);
+    v.shift = l - 1;
+    return v;
+}
+// floor division towards -inf: with s = n >> 63 (all ones for n < 0), n ^ s = -n - 1 >= 0 and floor(n / d) = ~floor((-n - 1) / d)
+__device__ __forceinline__ long long floor_div(long long n, const Divisor &d) {
+    const unsigned long long s = (unsigned long long)(n >> 63), u = (unsigned long long)n ^ s;
+    const unsigned long long q = d.magic ? __umul64hi(u, d.magic) >> d.shift : u;
+    return (long long)(q ^ s);
+}
+// the same for a compile-time divisor (the compiler's own multiply-high)
+template <unsigned long long D>
+__device__ __forceinline__ long long floor_div(long long n) {
+    const unsigned long long s = (unsigned long long)(n >> 63);
+    return (long long)((((unsigned long long)n ^ s) / D) ^ s);
+}
+
+// days since 1970-01-01 <-> proleptic Gregorian (year, month), 400-year eras of 146097 days counted from 0000-03-01
+__device__ __forceinline__ long long days_from_months(long long months) { // months since 1970-01 -> day of the month's first day
+    const long long yq = floor_div<12>(months);
+    const unsigned m = (unsigned)(months - yq * 12);     // 0 = January
+    const long long y = yq + 1970 - (m < 2);             // March-based year
+    const long long era = floor_div<400>(y);
+    const unsigned yoe = (unsigned)(y - era * 400);      // [0, 399]
+    const unsigned mp = m < 2 ? m + 10 : m - 2;          // 0 = March
+    const unsigned doe = yoe * 365 + yoe / 4 - yoe / 100 + (153 * mp + 2) / 5;
+    return era * 146097 + (long long)doe - 719468;
+}
+__device__ __forceinline__ long long months_from_days(long long days, bool years) { // -> months (or years) since 1970
+    const long long q = floor_div<146097>(days); // days + 719468 could overflow: shift the remainder instead
+    const unsigned z = (unsigned)(days - q * 146097) + 719468;
+    const long long era = q + z / 146097;
+    const unsigned doe = z % 146097;                                              // [0, 146096]
+    const unsigned yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;   // [0, 399]
+    const unsigned doy = doe - (365 * yoe + yoe / 4 - yoe / 100);                 // [0, 365], from March 1
+    const unsigned mp = (5 * doy + 2) / 153;                                      // 0 = March
+    const long long y = era * 400 + yoe + (mp >= 10) - 1970;
+    return years ? y : y * 12 + (mp < 10 ? mp + 2 : mp - 10);
+}
+
+// How a unit U becomes a resolution R.  Linear units (W .. ns) scale by one factor: p = floor(t * mul / div), one of mul, div 1.
+// CIVIL_IN (U = Y or M, R linear): t is first turned into the day its period starts on; CIVIL_OUT (U linear, R = M or Y): the
+// day count t * mul / div is turned into months or years.  Y <-> M is linear (x 12).  Multiplication wraps, as numpy's does.
+enum { TIME_CIVIL_IN = 1, TIME_CIVIL_OUT = 2, TIME_YEARS = 4 };
+struct TimeSteps {
+    int mode;
+    unsigned long long mul;
+    Divisor div;
+};
+// unit and resolution: b200_time_unit codes, both valid
+inline TimeSteps time_steps(int unit, int res) {
+    // nanoseconds per tick of W .. ns; Y and M have none
+    static const unsigned long long ns[B200_TIME_NUNITS] = {0, 0, 604800000000000ull, 86400000000000ull, 3600000000000ull, 60000000000ull,
+                                                           1000000000ull, 1000000ull, 1000ull, 1ull};
+    const bool civil_u = unit <= B200_TIME_M, civil_r = res <= B200_TIME_M;
+    TimeSteps s{0, 1, make_divisor(1)};
+    unsigned long long from, to;
+    if (civil_u && civil_r) { // months <-> years
+        from = unit == B200_TIME_Y ? 12 : 1;
+        to = res == B200_TIME_Y ? 12 : 1;
+    } else {
+        s.mode = civil_u ? TIME_CIVIL_IN | (unit == B200_TIME_Y ? TIME_YEARS : 0) : civil_r ? TIME_CIVIL_OUT | (res == B200_TIME_Y ? TIME_YEARS : 0) : 0;
+        from = ns[civil_u ? B200_TIME_D : unit];
+        to = ns[civil_r ? B200_TIME_D : res];
+    }
+    if (to >= from)
+        s.div = make_divisor(to / from);
+    else
+        s.mul = from / to;
+    return s;
+}
+__device__ __forceinline__ long long time_period(long long t, const TimeSteps &s) {
+    if (s.mode & TIME_CIVIL_IN)
+        t = days_from_months((s.mode & TIME_YEARS) ? (long long)((unsigned long long)t * 12) : t);
+    long long p = floor_div((long long)((unsigned long long)t * s.mul), s.div);
+    if (s.mode & TIME_CIVIL_OUT)
+        p = months_from_days(p, (s.mode & TIME_YEARS) != 0);
+    return p;
+}
+// the bin of one row: NaT and masked rows give -1 (the null cell through ordinal_index), like the reference's NaT // every
+__device__ __forceinline__ long long time_bin(long long t, bool masked, const TimeSteps &s, long long begin, const Divisor &every) {
+    if (masked || t == (long long)0x8000000000000000ULL)
+        return -1;
+    return floor_div((long long)((unsigned long long)time_period(t, s) - (unsigned long long)begin), every);
+}
+
 // ---- atomic cell updates -------------------------------------------------------------------------
 // float max/min on raw IEEE storage with integer atomics: non-negative floats order like signed ints,
 // negative floats order inversely as unsigned ints.  Works with the +-inf initial fill and is order independent.

@@ -15,6 +15,7 @@ from . import _lib
 from . import agg as _agg
 from . import execution, taskpart
 from . import hash as _hash
+from .groupby import Binner, BinnerBase, BinnerInteger, BinnerTime  # noqa: F401  (vaex.groupby's binners, for Frame.groupby)
 
 
 class Frame:
@@ -284,6 +285,21 @@ class Frame:
         if kind.strip() in ("%", "percent"):
             return self.limits_percentage(expression, ast.literal_eval(number), selection=selection)
         raise NotImplementedError(f"limits {value!r}: only 'minmax', 'N%' and explicit [min, max] pairs are supported")
+
+    def bin_edges(self, expression, limits, shape=128):
+        """df.bin_edges (vaex/dataframe.py:821-822): the shape + 1 edges of `shape` equal bins over `limits`"""
+        return self.bins(expression, limits, shape=shape, edges=True)
+
+    def bin_centers(self, expression, limits, shape=128):
+        """df.bin_centers (vaex/dataframe.py:824-825): the centers of `shape` equal bins over `limits`"""
+        return self.bins(expression, limits, shape=shape, edges=False)
+
+    def bins(self, expression, limits, shape=128, edges=True):
+        """df.bins (vaex/dataframe.py:827-835), numpy only: the bin edges, or the bin centers with edges=False"""
+        if edges:
+            return np.ogrid[limits[0]:limits[1]:(shape + 1) * 1j]
+        dx = (limits[1] - limits[0]) / shape
+        return np.ogrid[limits[0]:limits[1] - dx:(shape) * 1j] + dx / 2
 
     def limits_percentage(self, expression, percentage=99.73, square=False, selection=None):
         """df.limits_percentage (vaex/dataframe.py:1795-1842): a range around the median holding about `percentage` % of the rows, read
@@ -623,6 +639,8 @@ class Frame:
 
     # ---- groupby ------------------------------------------------------------------------------------------------------
     def groupby(self, by, agg=None, sort=False, fused=True, combine=False):
+        """df.groupby(by).agg(agg): `by` is a name, an expression, a binner (Binner, BinnerInteger, BinnerTime) or a list mixing them;
+        one output row per group with rows"""
         gb = GroupBy(self, by, sort=sort, fused=fused, combine=combine)
         return gb.agg(agg) if agg is not None else gb
 
@@ -640,14 +658,17 @@ class GroupBy:
         fewer than 10 rows per cell (vaex/groupby.py:653-668): the keys' ordinals are fused into one int64 code on the device
         (hash.CombinedCodes) and the groupby runs over the distinct codes — the reference's sparse `_combine` path
         (vaex/groupby.py:526-584)."""
-        self.by = [by] if isinstance(by, str) else list(by)
-        df = df._with_columns(self.by)  # a key that is an expression: group by it as a virtual column
+        self.by = [by] if isinstance(by, (str, BinnerBase)) else list(by)
+        binners = [b for b in self.by if isinstance(b, BinnerBase)]
+        df = df._with_columns([b.expression if isinstance(b, BinnerBase) else b for b in self.by])  # a key that is an expression: a virtual column
         self.df = df
         self.fused = fused
         self.sort = sort
         self.combined = None
         self.hash_maps = []
         for name in self.by:
+            if isinstance(name, BinnerBase):
+                continue
             col = df.columns[name]
             part = taskpart.TaskPartHashmapUniqueCreate(None, name, _lib.dtype_of(col), nthreads=1)
             # nthreads=1 -> 7 shards, chunks fed in row order: the ordinals of the sequential reference run
@@ -658,6 +679,11 @@ class GroupBy:
             if sort:
                 hm = hm.sorted()
             self.hash_maps.append(hm)
+        if binners:
+            # a binner's cells are fixed before the pass: the grid stays dense under combine="auto"
+            if combine is True and len(self.by) >= 2:
+                raise NotImplementedError(f"cannot combine {binners[0]!r} with other groupers: the sparse combine path takes hashed keys only")
+            return
         cells = 1
         for hm in self.hash_maps:
             cells *= len(hm)
@@ -714,7 +740,12 @@ class GroupBy:
         return self._decode(previous, level - 1) + ordinals[1:]
 
     def keys(self):
-        return [hm.keys() for hm in self.hash_maps]
+        return [k.bin_values if isinstance(k, BinnerBase) else hm.keys() for k, hm in zip(self.by, self._key_maps())]
+
+    def _key_maps(self):
+        """the hash map of every hashed key, None for a binner, in the order of `by`"""
+        maps = iter(self.hash_maps)
+        return [None if isinstance(k, BinnerBase) else next(maps) for k in self.by]
 
     def agg(self, actions):
         """actions: {column: [names]} | {column: name} | [descriptors]; returns dict of arrays (one row per non-empty group)."""
@@ -722,7 +753,8 @@ class GroupBy:
         descs, labels = [], []
         columns = dict(df.columns)
         if isinstance(actions, str):  # df.groupby(by, agg='count') (vaex/groupby.py:688-700)
-            actions = [_agg.aggregates[actions]("*")] if actions == "count" else {c: actions for c in df.columns if c not in self.by}
+            by = [k.expression if isinstance(k, BinnerBase) else k for k in self.by]
+            actions = [_agg.aggregates[actions]("*")] if actions == "count" else {c: actions for c in df.columns if c not in by}
         if isinstance(actions, dict):
             for col, names in actions.items():
                 if isinstance(names, _agg.AggregatorDescriptor):  # {'label': vaex.agg.mean('x')}: the key names the output column
@@ -761,7 +793,14 @@ class GroupBy:
                 out[label] = _take_cells(g, np.nonzero(keep)[0]) if _is_arrow(g) else g[:-2][keep]
             out["count"] = counts[keep]
             return out
-        for name, hm in zip(self.by, self.hash_maps):
+        # per key: its label, the cells of its grid axis, the first cell of a group and the group keys
+        axes = []
+        for name, hm in zip(self.by, self._key_maps()):
+            if hm is None:  # a binner: its cells are fixed (vaex_b200/groupby.py)
+                specs.append(name.spec(df))
+                axes.append((name.label, name.cells, name.start, name.bin_values))
+                continue
+            axes.append((name, len(hm) + 2, 0, hm.keys()))
             dtype = _lib.dtype_of(df.columns[name])
             if hm.is_string:
                 cname = f"_ordinal_values({name})"
@@ -778,17 +817,17 @@ class GroupBy:
         frame = df._derive(columns)
         grids = frame._agg(descs, binby=specs, edges=True)
         # _extract_center (vaex/groupby.py:896-977): drop the null / nan edge cells, keep groups with count > 0
-        center = tuple(slice(0, -2) for _ in self.by)
+        center = tuple(slice(start, start + len(keys)) for _, _, start, keys in axes)
         counts = grids[-1][center]
         keep = counts > 0
         out = {}
-        mesh = np.meshgrid(*[np.arange(len(hm)) for hm in self.hash_maps], indexing="ij")
-        for name, hm, m in zip(self.by, self.hash_maps, mesh):
-            out[name] = hm.keys()[m[keep]]
+        mesh = np.meshgrid(*[np.arange(len(keys)) for _, _, _, keys in axes], indexing="ij")
+        for (label, _, _, keys), m in zip(axes, mesh):
+            out[label] = keys[m[keep]]
         # a list aggregator returns ONE arrow list per cell of the flat FULL grid (first binner fastest, edge cells included)
-        shape = [len(hm) + 2 for hm in self.hash_maps]
+        shape = [cells for _, cells, _, _ in axes]
         strides = np.cumprod([1] + shape[:-1])
-        flat = sum(i.astype(np.int64) * int(st) for i, st in zip(np.nonzero(keep), strides))
+        flat = sum((i.astype(np.int64) + start) * int(st) for i, st, (_, _, start, _) in zip(np.nonzero(keep), strides, axes))
         for label, g in zip(labels[:-1], grids[:-1]):
             out[label] = _take_cells(g, flat) if _is_arrow(g) else g[center][keep]
         out["count"] = counts[keep]

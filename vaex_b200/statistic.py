@@ -134,9 +134,8 @@ class Statistic:
             ar, mask = _lib.split_mask(ar)
             if mask is not None:
                 mask = _lib.mask_column(mask)
-            if not _lib.is_device(ar) and np.asarray(ar).dtype.kind in "mM":  # the signed count of units, as numpy's astype(float) reads it
-                ar = np.asarray(ar)
-                ar = ar.view(np.dtype(np.int64).newbyteorder(ar.dtype.byteorder))
+            if _lib.dtype_of(ar).kind in "mM":  # the signed count of units, as numpy's astype(float) reads it
+                ar = _lib.int64_view(ar)
             c = _lib.column(ar)
             if c.length != nrows:
                 raise RuntimeError(f"expected a block of {nrows} rows, got {c.length}")

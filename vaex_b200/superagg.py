@@ -163,6 +163,52 @@ class _BinnerHash(Binner):
         return [col] + ([m] if m is not None else [])
 
 
+class _BinnerTime(Binner):
+    """``BinnerTime_int64(threads, expression, unit, resolution, begin, count, every)``: the reference's BinnerTime expression
+    ``(t.astype('M8[resolution]') - begin).astype('int') // every`` (vaex/groupby.py:118-126) fed to ``BinnerOrdinal(count)``, computed
+    in the binning kernel from the raw int64 ticks of a datetime64[unit] column.  An extension: the reference has no such class.
+    ``unit`` and ``resolution`` are numpy unit names (Y M W D h m s ms us ns); NaT, masked rows and periods outside the ``count``
+    bins fall into the null cell ``count``."""
+    _dtype = None
+    _non_native = False
+
+    def __init__(self, threads, expression, unit, resolution, begin, count, every=1):
+        super().__init__(threads, expression)
+        if unit not in _lib.TIME_UNITS or resolution not in _lib.TIME_UNITS:
+            raise ValueError(f"datetime units must be one of {_lib.TIME_UNITS}, not {unit!r} / {resolution!r}")
+        self.unit, self.resolution = unit, resolution
+        self.begin, self.ordinal_count, self.every = int(begin), int(count), int(every)
+
+    def _args(self):
+        return (self.threads, self.expression, self.unit, self.resolution, self.begin, self.ordinal_count, self.every)
+
+    def copy(self):
+        return type(self)(*self._args())
+
+    def __len__(self):
+        return self.ordinal_count + 2
+
+    def __reduce__(self):
+        return type(self), self._args()
+
+    def __repr__(self):
+        return f"<{type(self).__name__} expression={self.expression!r} M8[{self.unit}] -> M8[{self.resolution}] begin={self.begin} count={self.ordinal_count} every={self.every}>"
+
+    def _fill(self, b, thread):
+        col = self._data.get(thread)
+        if col is None:
+            raise RuntimeError("data not set")
+        b.kind = _lib.BINNER_TIME
+        b.dtype = self._code
+        b.byteswap = int(self._non_native)
+        b.reserved = _lib.TIME_UNITS.index(self.unit) | _lib.TIME_UNITS.index(self.resolution) << 8
+        b.ordinal_count, b.min_value, b.bins = self.ordinal_count, self.begin, self.every
+        b.data = col.ptr
+        m = self._mask.get(thread)
+        b.mask = m.ptr if m is not None else None
+        return [col] + ([m] if m is not None else [])
+
+
 class BinnerCombined:
     """``vaex.superagg.BinnerCombined(threads, binners)`` (src/binner_combined.cpp:5-36): a binner made of several binners whose
     indices are composed with strides 1, shape_0, shape_0 * shape_1, ... (``to_bins`` :25-29).  The reference binds it WITHOUT the
@@ -490,6 +536,8 @@ for _name in _DT:
         _make("BinnerScalar_" + _sfx, _BinnerScalar, **_common)
         _make("BinnerOrdinal_" + _sfx, _BinnerOrdinal, **_common)
         _make("BinnerHash_" + _sfx, _BinnerHash, **_common)
+        if _name == "int64":
+            _make("BinnerTime_" + _sfx, _BinnerTime, **_common)
         for _prefix, _op in _AGG_OPS.items():
             _make(_prefix + "_" + _sfx, Aggregator, _op=_op, **_common)
         _make("AggNUnique_" + _sfx, _AggNUnique, **_common)

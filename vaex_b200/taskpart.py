@@ -50,6 +50,12 @@ def decode_binner(spec, nthreads, hash_maps=None):
         if not isinstance(hm, _hash.HashMapUnique):
             hm = (hash_maps or {})[hm]
         return cls(nthreads, spec["expression"], hm)
+    if kind == "time":  # a datetime64[unit] column (its ticks as int64) -> periods of `resolution` (vaex_b200/groupby.py BinnerTime)
+        unit, step = np.datetime_data(dtype)
+        if dtype.kind != "M" or step != 1:
+            raise ValueError(f"a time binner needs a datetime64 column with a plain unit, not {dtype}")
+        cls = _agg.find_type_from_dtype(superagg, "BinnerTime_", np.dtype("int64").newbyteorder(dtype.byteorder))
+        return cls(nthreads, spec["expression"], unit, spec["resolution"], spec["begin"], spec["count"], spec.get("every", 1))
     raise ValueError("Cannot deserialize: %r" % spec)
 
 
