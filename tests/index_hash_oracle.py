@@ -9,14 +9,21 @@
 For one ``update`` at ``start_index=0``, and for several calls with increasing ``start_index`` and no NaN / null, this is what the
 reference computes.  Elsewhere the reference differs (DESIGN.md, index_hash): its NaN / null row is call-local, a merge drops the
 other index's NaN / null row, does not set has_duplicates by itself and appends the overflow in merge order.
+
+``IndexHash(dtype, nmaps, bits=True)`` keys floats by their canonical bit pattern (set_cases.canon), as the device does: -0.0 and 0.0
+are two keys there.  Lookups are first cast by value to the index's dtype, as the host's map_index does.  The default keys by Python
+``==`` (so -0.0 == 0.0), which is what the reference's std::equal_to does.
 """
 import numpy as np
 
+from set_cases import canon
+
 
 class IndexHash:
-    def __init__(self, dtype, nmaps=1):
+    def __init__(self, dtype, nmaps=1, bits=False):
         self.dtype = np.dtype(dtype)
         self.nmaps = nmaps
+        self.bits = bits
         self.rows = {}  # key -> every row, unsorted
         self.nan_count = self.null_count = 0
         self.nan_row = self.null_row = None
@@ -28,11 +35,20 @@ class IndexHash:
                 a = a.astype(self.dtype)  # update force-casts (py::array_t<T> forcecast)
         return a
 
+    def _hashable(self, a):
+        """the dict keys of a key array: its values, or in bit-pattern mode the canonical patterns of its values in the index's dtype"""
+        if not self.bits:
+            return a.tolist()
+        if a.dtype != self.dtype:
+            with np.errstate(invalid="ignore", over="ignore"):
+                a = a.astype(self.dtype)
+        return canon(a).tolist()
+
     def update(self, values, mask=None, start_index=0):
         a = self._keys(values)
         isnan = np.isnan(a) if a.dtype.kind == "f" else np.zeros(len(a), bool)
         m = np.zeros(len(a), bool) if mask is None else np.asarray(mask).astype(bool)
-        for i, (k, nan, masked) in enumerate(zip(a.tolist(), isnan.tolist(), m.tolist())):
+        for i, (k, nan, masked) in enumerate(zip(self._hashable(a), isnan.tolist(), m.tolist())):
             row = start_index + i
             if masked:
                 self.null_count += 1
@@ -74,7 +90,7 @@ class IndexHash:
         m = np.zeros(len(a), bool) if mask is None else np.asarray(mask).astype(bool)
         out = np.full(len(a), -1, np.int64)
         unknown = False
-        for i, (k, nan, masked) in enumerate(zip(a.tolist(), isnan.tolist(), m.tolist())):
+        for i, (k, nan, masked) in enumerate(zip(self._hashable(a), isnan.tolist(), m.tolist())):
             if nan:
                 v = self.nan_row if self.nan_count else -1
             elif masked:
@@ -94,7 +110,7 @@ class IndexHash:
         isnan = np.isnan(a) if a.dtype.kind == "f" else np.zeros(len(a), bool)
         m = np.zeros(len(a), bool) if mask is None else np.asarray(mask).astype(bool)
         left, right = [], []
-        for i, (k, nan, masked) in enumerate(zip(a.tolist(), isnan.tolist(), m.tolist())):
+        for i, (k, nan, masked) in enumerate(zip(self._hashable(a), isnan.tolist(), m.tolist())):
             if nan or masked or k not in self.rows:
                 continue
             extra = sorted(self.rows[k])[1:]
@@ -103,7 +119,8 @@ class IndexHash:
         return np.array(left, np.int64), np.array(right, np.int64)
 
     def extract(self):
-        """{key: primary row} over all shards (the shard split is the reference's hash; compare the union)"""
+        """{key: primary row} over all shards (the shard split is the reference's hash; compare the union); in bit-pattern mode the
+        keys are canonical patterns"""
         return {k: min(r) for k, r in self.rows.items()}
 
 
@@ -134,5 +151,5 @@ class RefAPI(IndexHash):
         return self._write(*IndexHash.map_index(self, values, mask), out)
 
 
-def classes(dtype):
-    return lambda nmaps=1: RefAPI(dtype, nmaps)
+def classes(dtype, bits=False):
+    return lambda nmaps=1: RefAPI(dtype, nmaps, bits)

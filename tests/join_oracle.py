@@ -92,7 +92,9 @@ def mangle_name(prefix, name, suffix):
     return prefix + name + suffix
 
 
-def join(df, other, on=None, left_on=None, right_on=None, lprefix='', rprefix='', lsuffix='', rsuffix='', how='left', allow_duplication=False):
+def join(df, other, on=None, left_on=None, right_on=None, lprefix='', rprefix='', lsuffix='', rsuffix='', how='left', allow_duplication=False,
+         bits=False):
+    """`bits`: key the index by bit pattern, the device's rule (index_hash_oracle.IndexHash)"""
     inner = False
     left, right = df, other
     if how == 'left':
@@ -120,7 +122,7 @@ def join(df, other, on=None, left_on=None, right_on=None, lprefix='', rprefix=''
     lookup = None
     if left_on is not None or right_on is not None:
         keys, mask = _keys(right.columns[right_on])
-        index = IndexHash(keys.dtype)
+        index = IndexHash(keys.dtype, bits=bits)
         index.update(keys, mask)
         if index.has_duplicates and not allow_duplication:
             raise ValueError('This join will lead to duplication of rows which is disabled, pass allow_duplication=True')

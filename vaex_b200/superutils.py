@@ -297,6 +297,18 @@ for _name in _lib.DTYPES:
     globals()["counter_" + _name] = _cls
 
 
+def device_cast(keys, dtype, ctx):
+    """a device key column of another dtype as `dtype`, cast by value where numpy would cast it safely; anything else is a TypeError"""
+    import torch
+    have = _lib.dtype_of(keys)
+    if not np.can_cast(have, dtype, "safe"):
+        raise TypeError(f"map_index: incompatible key dtype {have} (index dtype {dtype})")
+    ctx.sync()  # a device expression's block is written on a slot's stream
+    out = torch.as_tensor(keys, device=f"cuda:{ctx.device}").to(getattr(torch, dtype.name))
+    torch.cuda.synchronize(out.device)  # the cast runs on torch's stream, the lookup on a slot's
+    return out
+
+
 _INDEX_OUT = {np.dtype(t): np.dtype(t).itemsize for t in ("int8", "int16", "int32", "int64")}
 
 
@@ -324,12 +336,19 @@ class _IndexHash:
 
     def _lookup_column(self, values):
         """map_index takes ``py::array_t<T>`` without forcecast: numpy converts only where the cast is safe (int32 keys on an int64
-        index), anything else is a TypeError.  Device columns follow ``_key_column``."""
+        index), anything else is a TypeError.  Device columns follow the same rule: one of another dtype is cast by value on the
+        device where numpy calls that safe, and refused otherwise, so a key never reads differently on the host and the device (int8
+        -1 is not 255 on a uint8 index, uint64 2^63 not INT64_MIN on an int64 one)."""
         native = self._np_dtype()
-        if isinstance(values, np.ndarray) and not np.can_cast(values.dtype, native, "safe"):
-            raise TypeError(f"{type(self).__name__}.map_index: incompatible key dtype {values.dtype} (index dtype {native})")
-        if not isinstance(values, np.ndarray) and getattr(values, "__cuda_array_interface__", None) is None:
+        if _lib.is_device(values):
+            have = _lib.dtype_of(values)
+            if have == native:
+                return self._key_column(values)
+            return self._key_column(device_cast(values, native, self._ctx))
+        if not isinstance(values, np.ndarray):
             values = np.asarray(values, dtype=native)
+        if not np.can_cast(values.dtype, native, "safe"):
+            raise TypeError(f"{type(self).__name__}.map_index: incompatible key dtype {values.dtype} (index dtype {native})")
         return self._key_column(values)
 
     def _info(self):

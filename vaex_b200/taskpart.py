@@ -19,6 +19,7 @@ from . import _lib
 from . import agg as _agg
 from . import hash as _hash
 from . import superagg
+from . import superutils
 
 
 def _issequence(x):
@@ -375,9 +376,9 @@ class TaskPartLookup(TaskPart):
     def process(self, thread_index, i1, i2, filter_mask, selection_masks, blocks):
         keys, mask = _key_block(blocks[0])
         native = self.index._np_dtype()
-        if _lib.is_device(keys) and _lib.dtype_of(keys) != native:
-            keys = _device_cast(keys, native, self._ctx)
         slot = self._ctx.slot(thread_index)
+        if _lib.is_device(keys) and _lib.dtype_of(keys) != native:
+            keys = superutils.device_cast(keys, native, self._ctx)  # once for map_index and map_index_duplicates
         out = self.lookup[i1:i2]
         if mask is None:
             unknown = self.index.map_index(keys, out, slot=slot)
@@ -394,18 +395,6 @@ class TaskPartLookup(TaskPart):
 
     def get_result(self):
         return self.unknown, self.extra
-
-
-def _device_cast(keys, dtype, ctx):
-    """a device key column of another dtype as `dtype`, where numpy would cast it safely (map_index refuses the rest)"""
-    import torch
-    have = _lib.dtype_of(keys)
-    if not np.can_cast(have, dtype, "safe"):
-        raise TypeError(f"map_index: incompatible key dtype {have} (index dtype {dtype})")
-    ctx.sync()  # a device expression's block is written on a slot's stream
-    out = torch.as_tensor(keys, device=f"cuda:{ctx.device}").to(getattr(torch, dtype.name))
-    torch.cuda.synchronize(out.device)  # the cast runs on torch's stream, the lookup on a slot's
-    return out
 
 
 class TaskPartStatistic(TaskPart):
