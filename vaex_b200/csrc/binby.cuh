@@ -7,15 +7,9 @@
 
 #include "common.cuh"
 #include "device_utils.cuh"
+#include "settable.cuh"
 
 namespace b200 {
-
-// open-addressing slot of the device ordered_set (hashset.cu)
-#define SET_EMPTY 0xFFFFFFFFFFFFFFFFULL
-struct SetSlot {
-    unsigned long long key;   // canonical 64-bit key pattern
-    unsigned long long first; // pass 1: (chunk_seq << 40 | row) of the first occurrence; after finalize: global ordinal
-};
 
 struct DevBinner {
     int kind, dtype, isz, byteswap, allow_other, invert;

@@ -2,24 +2,9 @@
 #pragma once
 #include "binby.cuh"
 #include "device_utils.cuh"
+#include "settable.cuh"
 
 namespace b200 {
-
-// probe of the finalized ordered_set table (ordered_set::_map_ordinal, src/hash_primitives.hpp:624-691)
-__device__ __forceinline__ long long set_probe(const SetSlot *table, unsigned long long mask, long long sentinel_ordinal, uint64_t canon) {
-    if (canon == SET_EMPTY)
-        return sentinel_ordinal;
-    unsigned long long h = hash64(canon) & mask;
-    while (true) {
-        // one 16-byte load per probe: key and ordinal share a sector
-        const ulonglong2 s = __ldg(reinterpret_cast<const ulonglong2 *>(table + h));
-        if (s.x == canon)
-            return (long long)s.y;
-        if (s.x == SET_EMPTY)
-            return -1;
-        h = (h + 1) & mask;
-    }
-}
 
 template <bool VEC>
 __device__ __forceinline__ void binby_indices(const DevBinner *__restrict__ binners, int nb, long long base, int nv, unsigned long long idx[4]) {
@@ -64,7 +49,7 @@ __device__ __forceinline__ void binby_indices(const DevBinner *__restrict__ binn
                 else if (raw_isnan(b.dtype, raw))
                     value = b.nan_ordinal;
                 else
-                    value = set_probe(b.table, b.table_mask, b.sentinel_ordinal, key_canon(b.dtype, raw));
+                    value = set_ordinal(b.table, b.table_mask, b.sentinel_ordinal, key_canon(b.dtype, raw));
                 idx[j] += ordinal_index(value, false, b.ordinal_count, b.allow_other != 0, b.invert != 0) * b.stride;
             }
         }

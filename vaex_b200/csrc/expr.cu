@@ -18,6 +18,7 @@
 #include "binby.cuh"
 #include "device_utils.cuh"
 #include "scan.cuh"
+#include "settable.cuh"
 
 namespace b200 {
 int set_fill_binner(b200_set *s, DevBinner &b); // hashset.cu
@@ -177,18 +178,7 @@ __device__ __forceinline__ long long ordinal_lookup(const EvalParams &p, int k, 
         }
     }
     (void)cls;
-    const uint64_t canon = key_canon(dt, raw);
-    if (canon == SET_EMPTY)
-        return p.sentinel_ordinal[k];
-    unsigned long long h = hash64(canon) & p.table_mask[k];
-    while (true) {
-        const ulonglong2 s = __ldg(reinterpret_cast<const ulonglong2 *>(p.table[k] + h));
-        if (s.x == canon)
-            return (long long)s.y;
-        if (s.x == SET_EMPTY)
-            return -1;
-        h = (h + 1) & p.table_mask[k];
-    }
+    return set_ordinal(p.table[k], p.table_mask[k], p.sentinel_ordinal[k], key_canon(dt, raw));
 }
 
 __global__ void __launch_bounds__(256) k_eval(const __grid_constant__ EvalParams p) {

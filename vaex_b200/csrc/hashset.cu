@@ -18,6 +18,7 @@
 #include "device_utils.cuh"
 #include "radix.cuh"
 #include "scan.cuh"
+#include "settable.cuh"
 #include "strings.cuh"
 
 namespace b200 {
@@ -90,35 +91,6 @@ constexpr unsigned long long kTagLowMask = (1ULL << 40) - 1;
 __host__ __device__ __forceinline__ unsigned long long index_bias(long long row) { return (unsigned long long)row ^ (1ull << 63); }
 __host__ __device__ __forceinline__ long long index_unbias(unsigned long long tag) { return (long long)(tag ^ (1ull << 63)); }
 
-// insert (or touch) one key; returns false when the table is too full.  "Too full" is detected by PROBE LENGTH, not by a fill
-// counter: one shared counter bumped per new key serialises in the L2 (one update at a time to one address), while a
-// linear-probing table at load <= 0.5 practically never needs more than
-// kMaxProbe steps and one past ~0.85 quickly does.  The bound also makes every probe loop finite by construction.
-constexpr int kMaxProbe = 96;
-__device__ __forceinline__ bool table_insert(SetSlot *table, unsigned long long mask, unsigned long long canon, unsigned long long tag) {
-    unsigned long long h = hash64(canon) & mask;
-    for (int step = 0; step < kMaxProbe; step++) {
-        // ONE 16-byte L2 load per probe: key and tag share a sector.  A stale tag is harmless: tags only decrease, so at worst the
-        // atomicMin below is issued although it changes nothing
-        const ulonglong2 slot = __ldcg(reinterpret_cast<const ulonglong2 *>(table + h));
-        unsigned long long k = slot.x;
-        unsigned long long first = slot.y;
-        if (k == SET_EMPTY) {
-            k = atomicCAS(&table[h].key, SET_EMPTY, canon);
-            if (k == SET_EMPTY)
-                k = canon;
-            first = ~0ull;
-        }
-        if (k == canon) {
-            if (tag < first)
-                atomicMin(&table[h].first, tag);
-            return true;
-        }
-        h = (h + 1) & mask;
-    }
-    return false;
-}
-
 // hash_base::_update (src/hash_primitives.hpp:98-295).  from_keys: ordered_set::create (:486-537) where row i IS the ordinal.
 __global__ void __launch_bounds__(256) k_set_insert(SetSlot *table, unsigned long long mask, unsigned long long *ctr, int dtype,
                                                     int isz, const void *keys, const uint8_t *masks, long long row0, long long nrows,
@@ -130,8 +102,8 @@ __global__ void __launch_bounds__(256) k_set_insert(SetSlot *table, unsigned lon
     unsigned long long n_nan = 0, n_null = 0, t_nan = ~0ull, t_null = ~0ull;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
         // once the table overflowed this launch will be redone after a growth: stop inserting (and stop altogether on a redo,
-        // whose NaN/null rows were already counted); the flag is polled every 32 rows per thread
-        if (!dead && (it++ & 31) == 0 && *reinterpret_cast<volatile unsigned long long *>(ctr + CTR_OVERFLOW))
+        // whose NaN/null rows were already counted)
+        if (!dead && (it++ % kPollRows) == 0 && overflow_seen(ctr + CTR_OVERFLOW))
             dead = true;
         if (dead && (skip_keys & 2))
             return;
@@ -160,11 +132,8 @@ __global__ void __launch_bounds__(256) k_set_insert(SetSlot *table, unsigned lon
             atomicMin(ctr + CTR_SENTINEL_TAG, tag);
             continue;
         }
-        if (!table_insert(table, mask, canon, tag)) {
-            // raise the flag ONCE (millions of plain stores to one address serialise in the L2) and stop: the host grows the table
-            // and redoes this range
-            if (!*reinterpret_cast<volatile unsigned long long *>(ctr + CTR_OVERFLOW))
-                ctr[CTR_OVERFLOW] = 1ull;
+        if (!set_insert(table, mask, canon, tag)) { // the host grows the table and redoes this range
+            overflow_raise(ctr + CTR_OVERFLOW);
             dead = true;
         }
     }
@@ -193,19 +162,9 @@ __global__ void __launch_bounds__(256) k_set_count(const SetSlot *table, unsigne
             n_sent += w;
             continue;
         }
-        // the key is present (the insert pass of these rows succeeded); a rehash may have placed it further than kMaxProbe from its
-        // home slot, so the probe is bounded by the empty slot only
-        unsigned long long h = hash64(canon) & mask;
-        while (true) {
-            const unsigned long long k = table[h].key;
-            if (k == canon) {
-                atomicAdd(counts + h, w);
-                break;
-            }
-            if (k == SET_EMPTY)
-                break;
-            h = (h + 1) & mask;
-        }
+        const unsigned long long h = set_slot(table, mask, canon); // present: the insert pass of these rows succeeded
+        if (h != ~0ull)
+            atomicAdd(counts + h, w);
     }
     if (n_sent)
         atomicAdd(ctr + CTR_SENTINEL_COUNT, n_sent);
@@ -218,10 +177,9 @@ __global__ void k_counts_gather(const SetSlot *table, unsigned long long cap, co
         const unsigned long long k = table[i].key;
         if (k == SET_EMPTY)
             continue;
-        unsigned long long h = hash64(k) & pmask;
-        while (probe[h].key != k)
-            h = (h + 1) & pmask;
-        out[probe[h].first] = counts[i];
+        const unsigned long long h = set_slot(probe, pmask, k); // present: every key of the table is in the probe table
+        if (h != ~0ull)
+            out[probe[h].first] = counts[i];
     }
 }
 
@@ -238,9 +196,7 @@ __global__ void k_set_rehash(const SetSlot *old, unsigned long long old_cap, Set
         unsigned long long k = old[i].key;
         if (k == SET_EMPTY)
             continue;
-        unsigned long long h = hash64(k) & mask;
-        while (atomicCAS(&table[h].key, SET_EMPTY, k) != SET_EMPTY)
-            h = (h + 1) & mask;
+        const unsigned long long h = set_claim(table, mask, k);
         table[h].first = old[i].first;
         if (counts)
             counts[h] = old_counts[i];
@@ -298,24 +254,7 @@ __global__ void k_set_finish(const unsigned long long *val, const unsigned long 
             continue; // the key whose pattern equals SET_EMPTY cannot live in the table either
         }
         keys_ord[i] = k;
-        unsigned long long h = hash64(k) & pmask;
-        while (atomicCAS(&probe[h].key, SET_EMPTY, k) != SET_EMPTY)
-            h = (h + 1) & pmask;
-        probe[h].first = i;
-    }
-}
-
-__device__ __forceinline__ long long probe_lookup(const SetSlot *probe, unsigned long long mask, long long sentinel_ordinal, unsigned long long canon) {
-    if (canon == SET_EMPTY)
-        return sentinel_ordinal;
-    unsigned long long h = hash64(canon) & mask;
-    while (true) {
-        const ulonglong2 s = __ldg(reinterpret_cast<const ulonglong2 *>(probe + h));
-        if (s.x == canon)
-            return (long long)s.y;
-        if (s.x == SET_EMPTY)
-            return -1;
-        h = (h + 1) & mask;
+        probe[set_claim(probe, pmask, k)].first = i;
     }
 }
 
@@ -324,7 +263,7 @@ __global__ void __launch_bounds__(256) k_set_map(const SetSlot *probe, unsigned 
                                                  int isz, const void *keys, long long nrows, void *out, int out_isz) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
         uint64_t raw = ldcs1_raw(keys, isz, i);
-        long long v = raw_isnan(dtype, raw) ? nan_ordinal : probe_lookup(probe, mask, sentinel_ordinal, key_canon(dtype, raw));
+        long long v = raw_isnan(dtype, raw) ? nan_ordinal : set_ordinal(probe, mask, sentinel_ordinal, key_canon(dtype, raw));
         if (out_isz)
             store1_raw(out, out_isz, i, (uint64_t)v);
         else
@@ -353,7 +292,7 @@ __global__ void __launch_bounds__(256) k_set_combine(const __grid_constant__ Com
                 o = p.null_ord[k];
             } else {
                 const uint64_t raw = ldcs1_raw(p.keys[k], p.isz[k], i);
-                o = raw_isnan(p.dtype[k], raw) ? p.nan_ord[k] : probe_lookup(p.probe[k], p.mask[k], p.sentinel[k], key_canon(p.dtype[k], raw));
+                o = raw_isnan(p.dtype[k], raw) ? p.nan_ord[k] : set_ordinal(p.probe[k], p.mask[k], p.sentinel[k], key_canon(p.dtype[k], raw));
             }
             missing |= o < 0;
             acc += o * p.mult[k];
@@ -377,7 +316,7 @@ __global__ void __launch_bounds__(256) k_set_values(const SetSlot *probe, unsign
         } else {
             unsigned long long canon = key_canon(dtype, raw);
             int shard = (int)(key_hash(dtype, canon) % (unsigned long long)nmaps);
-            long long g = probe_lookup(probe, mask, sentinel_ordinal, canon);
+            long long g = set_ordinal(probe, mask, sentinel_ordinal, canon);
             out_values[i] = g - offsets[shard];
             out_map[i] = (short)shard;
         }
@@ -425,10 +364,40 @@ int set_grow(b200_set *s, cudaStream_t st, uint64_t new_cap = 0) {
     return B200_OK;
 }
 
+// room for the worst case of a call that inserts `nrows` rows: every row a new key, capped at 2^22 slots = 64 MB.  One growth step
+// up front avoids the grow-and-redo cascade 4K -> 16K -> ... (five allocations and rehashes) on big inputs; growth on demand covers
+// the rest
+int set_reserve(b200_set *s, cudaStream_t st, int64_t nrows) {
+    const uint64_t known = s->dirty ? 0 : (uint64_t)s->n_keys; // exact only right after a finalisation
+    const uint64_t target = std::min<uint64_t>((known + (uint64_t)nrows) * 2, 1ull << 22);
+    uint64_t want = s->cap;
+    while (want < target)
+        want <<= 1;
+    return want > s->cap ? set_grow(s, st, want) : B200_OK;
+}
+
 int read_ctr(b200_set *s, cudaStream_t st, unsigned long long *h) {
     B200_CUDA(cudaMemcpyAsync(h, s->d_ctr, sizeof(unsigned long long) * CTR_N, cudaMemcpyDeviceToHost, st));
     B200_CUDA(cudaStreamSynchronize(st));
     return B200_OK;
+}
+
+// Runs one insert pass until the table holds it: pass(redo) enqueues the pass on `st` and returns its launch status.  When a
+// thread's insert overflowed, the table grows four-fold and the pass runs again with redo = 2: key inserts are idempotent (CAS claim
+// + atomicMin of the tag), while a pass's NaN / null counting is not and is skipped on a redo.  The loop ends when the pass fits or
+// when set_grow cannot allocate the larger table.
+template <typename Pass>
+int set_insert_pass(b200_set *s, cudaStream_t st, Pass &&pass) {
+    unsigned long long h[CTR_N];
+    for (int redo = 0;; redo = 2) {
+        B200_CHECK(pass(redo));
+        B200_CHECK(read_ctr(s, st, h));
+        if (!h[CTR_OVERFLOW])
+            return B200_OK;
+        unsigned long long zero = 0;
+        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_OVERFLOW, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
+        B200_CHECK(set_grow(s, st));
+    }
 }
 
 // the shard of a key is key_hash(dtype, key) % nmaps; a string set's table key already IS the reference's string hash, and the
@@ -446,7 +415,7 @@ int set_finalize(b200_set *s) {
     cudaStream_t st = s->ctx->slots[0]->stream;
     unsigned long long h[CTR_N];
     unsigned long long zero = 0;
-    // the insert kernel keeps no fill counter (see table_insert): count the occupied slots first, then compact them
+    // the insert kernel keeps no fill counter (see kMaxProbe in settable.cuh): count the occupied slots first, then compact them
     B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_CURSOR, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
     k_set_compact<<<nblocks(s->cap), 256, 0, st>>>(s->table, s->cap, s->d_ctr, nullptr, nullptr, nullptr, shard_dtype(s), s->nmaps);
     B200_CHECK(read_ctr(s, st, h));
@@ -574,7 +543,6 @@ int64_t set_count_locked(b200_set *s) { return s->n_keys + (s->nan_count > 0) + 
 // insert rows [0, nrows) of device arrays; caller holds s->mu
 int set_insert_device(b200_set *s, cudaStream_t st, const void *d_keys, const uint8_t *d_masks, int64_t nrows, bool use_offsets, bool from_keys,
                       int64_t from_keys_null_index, int64_t start_index = 0) {
-    unsigned long long h[CTR_N];
     int skip_keys = 0;
     if (s->limit >= 0) { // hash_primitives.hpp:237-249: a full set skips the whole flush of this call
         B200_CHECK(set_finalize(s));
@@ -589,33 +557,15 @@ int set_insert_device(b200_set *s, cudaStream_t st, const void *d_keys, const ui
     const unsigned long long nan_low = use_offsets ? second_low : first_low;
     const int isz = dtype_size(s->dtype);
     const int64_t sub = 1ll << 26;
-    // size the table for the call up front (every row could be a new key, capped at 2^22 slots = 64 MB): avoids the
-    // grow-and-redo cascade 4K -> 16K -> ... on big inputs; further growth still happens on demand
-    {
-        uint64_t want = s->cap;
-        const uint64_t known = s->dirty ? 0 : (uint64_t)s->n_keys; // exact only right after a finalisation; growth on demand covers the rest
-        const uint64_t target = std::min<uint64_t>((known + (uint64_t)nrows) * 2, 1ull << 22);
-        while (want < target)
-            want <<= 1;
-        if (s->cap < want)
-            B200_CHECK(set_grow(s, st, want)); // one step (the cascade 4K -> 16K -> ... cost five allocations and rehashes)
-    }
-    int redo = 0;
-    for (int64_t row0 = 0; row0 < nrows;) {
-        int64_t n = std::min<int64_t>(sub, nrows - row0);
-        k_set_insert<<<nblocks((unsigned long long)n), 256, 0, st>>>(s->table, s->cap - 1, s->d_ctr, s->dtype, isz, d_keys, d_masks, row0, n,
-                                                                     tag_base, skip_keys | redo, from_keys_null_index, from_keys ? 1 : 0, nan_low, null_low);
-        B200_CUDA(cudaGetLastError());
-        B200_CHECK(read_ctr(s, st, h));
-        if (h[CTR_OVERFLOW]) {
-            unsigned long long zero = 0;
-            B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_OVERFLOW, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
-            B200_CHECK(set_grow(s, st));
-            redo = 2; // redo this range: key inserts are idempotent (CAS claim + atomicMin of the tag); NaN/null counting is not
-            continue;
-        }
-        redo = 0;
-        row0 += n;
+    B200_CHECK(set_reserve(s, st, nrows));
+    for (int64_t row0 = 0; row0 < nrows; row0 += sub) {
+        const int64_t n = std::min<int64_t>(sub, nrows - row0);
+        B200_CHECK(set_insert_pass(s, st, [&](int redo) -> int {
+            k_set_insert<<<nblocks((unsigned long long)n), 256, 0, st>>>(s->table, s->cap - 1, s->d_ctr, s->dtype, isz, d_keys, d_masks, row0, n, tag_base,
+                                                                         skip_keys | redo, from_keys_null_index, from_keys ? 1 : 0, nan_low, null_low);
+            B200_CUDA(cudaGetLastError());
+            return B200_OK;
+        }));
     }
     if (s->counting && !s->hold_count_pass && !skip_keys && nrows) {
         k_set_count<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->table, s->cap - 1, s->counts, s->d_ctr, s->dtype, isz, d_keys, d_masks, nullptr, nrows);
@@ -665,20 +615,9 @@ __global__ void __launch_bounds__(256) k_index_log(unsigned long long *ctr, int 
         atomicMax(ctr + CTR_NULL_MAX, null_max);
 }
 
-// the slot of a key known to be present (a rehash may have placed it past kMaxProbe: bounded by the empty slot only); the key whose
-// pattern is SET_EMPTY lives outside the table, at slot `cap`
+// the slot of a key (~0ull: absent); the key whose pattern is SET_EMPTY lives outside the table, at slot `cap`
 __device__ __forceinline__ unsigned long long index_slot(const SetSlot *table, unsigned long long mask, unsigned long long canon) {
-    if (canon == SET_EMPTY)
-        return mask + 1;
-    unsigned long long h = hash64(canon) & mask;
-    while (true) {
-        const unsigned long long k = table[h].key;
-        if (k == canon)
-            return h;
-        if (k == SET_EMPTY)
-            return ~0ull;
-        h = (h + 1) & mask;
-    }
+    return canon == SET_EMPTY ? mask + 1 : set_slot(table, mask, canon);
 }
 
 // radix input: sort key = row - row_min, payload = slot << 32 (the shard-pass layout of radix.cuh: from_val digits)
@@ -734,24 +673,14 @@ __global__ void __launch_bounds__(256) k_index_map(const SetSlot *table, unsigne
             unk |= v == -1;
         } else {
             const unsigned long long canon = key_canon(dtype, raw);
-            bool found = false;
-            v = -1;
+            bool found;
             if (canon == SET_EMPTY) {
                 found = sp.sent_present;
                 v = sp.sent_row;
             } else {
-                unsigned long long h = hash64(canon) & mask;
-                while (true) {
-                    const ulonglong2 s = __ldg(reinterpret_cast<const ulonglong2 *>(table + h));
-                    if (s.x == canon) {
-                        found = true;
-                        v = index_unbias(s.y);
-                        break;
-                    }
-                    if (s.x == SET_EMPTY)
-                        break;
-                    h = (h + 1) & mask;
-                }
+                unsigned long long first;
+                found = set_lookup(table, mask, canon, &first);
+                v = found ? index_unbias(first) : -1;
             }
             unk |= !found;
         }
@@ -816,8 +745,8 @@ __global__ void __launch_bounds__(256) k_index_merge_table(const SetSlot *other,
         const SetSlot s = other[i];
         if (s.key == SET_EMPTY)
             continue;
-        if (!table_insert(table, mask, s.key, s.first)) {
-            ctr[CTR_OVERFLOW] = 1ull;
+        if (!set_insert(table, mask, s.key, s.first)) {
+            overflow_raise(ctr + CTR_OVERFLOW);
             return;
         }
     }
@@ -936,16 +865,11 @@ int index_merge_one(b200_set *s, b200_set *o, cudaStream_t st) {
         want <<= 1;
     if (want > s->cap)
         B200_CHECK(set_grow(s, st, want));
-    while (true) {
+    B200_CHECK(set_insert_pass(s, st, [&](int) -> int {
         k_index_merge_table<<<nblocks(o->cap), 256, 0, st>>>(o->table, o->cap, s->table, s->cap - 1, s->d_ctr);
         B200_CUDA(cudaGetLastError());
-        B200_CHECK(read_ctr(s, st, h));
-        if (!h[CTR_OVERFLOW])
-            break;
-        unsigned long long zero = 0;
-        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_OVERFLOW, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
-        B200_CHECK(set_grow(s, st));
-    }
+        return B200_OK;
+    }));
     B200_CHECK(index_log_reserve(s, st, s->log_n + o->log_n));
     if (o->log_n) {
         B200_CUDA(cudaMemcpyAsync(s->log_key + s->log_n, o->log_key, o->log_n * 8, cudaMemcpyDeviceToDevice, st));
@@ -1636,7 +1560,7 @@ __global__ void __launch_bounds__(256) k_str_insert(SetSlot *table, unsigned lon
     bool dead = false;
     unsigned it = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += (long long)gridDim.x * blockDim.x) {
-        if (!dead && (it++ & 31) == 0 && *reinterpret_cast<volatile unsigned long long *>(ctr + CTR_OVERFLOW))
+        if (!dead && (it++ % kPollRows) == 0 && overflow_seen(ctr + CTR_OVERFLOW))
             dead = true;
         if (dead && (skip & 2))
             return;
@@ -1658,34 +1582,15 @@ __global__ void __launch_bounds__(256) k_str_insert(SetSlot *table, unsigned lon
             continue;
         }
         const unsigned long long tag = tag_base | (unsigned long long)row;
-        unsigned long long pos = hash64(h) & mask;
-        bool done = false;
-        for (int step = 0; step < kMaxProbe && !done; step++) {
-            const ulonglong2 slot = __ldcg(reinterpret_cast<const ulonglong2 *>(table + pos));
-            unsigned long long k = slot.x, first = slot.y;
-            if (k == SET_EMPTY) {
-                k = atomicCAS(&table[pos].key, SET_EMPTY, h);
-                if (k == SET_EMPTY) { // this thread owns the new key: pool its bytes, log it
-                    k = h;
-                    first = ~0ull;
-                    const unsigned long long li = atomicAdd(strctr + 0, 1ull), po = atomicAdd(strctr + 1, len);
-                    for (unsigned long long c = 0; c < len; c++)
-                        pool[po + c] = (char)bytes[b + c];
-                    log[li].hash = h, log[li].off = po, log[li].len = (unsigned)len;
-                    slot_log[pos] = (unsigned)li;
-                }
-            }
-            if (k == h) {
-                if (tag < first)
-                    atomicMin(&table[pos].first, tag);
-                done = true;
-            } else {
-                pos = (pos + 1) & mask;
-            }
-        }
-        if (!done) {
-            if (!*reinterpret_cast<volatile unsigned long long *>(ctr + CTR_OVERFLOW))
-                ctr[CTR_OVERFLOW] = 1ull;
+        auto pool_key = [&](unsigned long long slot) { // this thread owns the new key: pool its bytes, log it
+            const unsigned long long li = atomicAdd(strctr + 0, 1ull), po = atomicAdd(strctr + 1, len);
+            for (unsigned long long c = 0; c < len; c++)
+                pool[po + c] = (char)bytes[b + c];
+            log[li].hash = h, log[li].off = po, log[li].len = (unsigned)len;
+            slot_log[slot] = (unsigned)li;
+        };
+        if (!set_insert(table, mask, h, tag, pool_key)) {
+            overflow_raise(ctr + CTR_OVERFLOW);
             dead = true;
         }
     }
@@ -1714,26 +1619,19 @@ __global__ void __launch_bounds__(256) k_str_verify(const SetSlot *table, unsign
         const unsigned long long h = murmur64(bytes + b, len);
         if (h == SET_EMPTY)
             continue;
-        unsigned long long pos = hash64(h) & mask;
-        while (true) {
-            const unsigned long long k = table[pos].key;
-            if (k == h) {
-                const StrLog r = log[slot_log[pos]];
-                if (r.len != len || !bytes_equal(pool + r.off, bytes + b, len))
-                    ctr[CTR_STR_ERROR] = 2;
-                break;
-            }
-            if (k == SET_EMPTY)
-                break; // cannot happen after a successful insert pass
-            pos = (pos + 1) & mask;
-        }
+        const unsigned long long pos = set_slot(table, mask, h);
+        if (pos == ~0ull)
+            continue; // cannot happen after a successful insert pass
+        const StrLog r = log[slot_log[pos]];
+        if (r.len != len || !bytes_equal(pool + r.off, bytes + b, len))
+            ctr[CTR_STR_ERROR] = 2;
     }
 }
 
 // finalized view: ordinal -> where the key's bytes are
 __global__ void k_str_index(const StrLog *log, unsigned long long nlog, const SetSlot *probe, unsigned long long pmask, unsigned long long *str_off, unsigned *str_len) {
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nlog; i += (unsigned long long)gridDim.x * blockDim.x) {
-        const long long ord = probe_lookup(probe, pmask, -1, log[i].hash);
+        const long long ord = set_ordinal(probe, pmask, -1, log[i].hash);
         if (ord >= 0) {
             str_off[ord] = log[i].off;
             str_len[ord] = log[i].len;
@@ -1756,7 +1654,7 @@ __global__ void __launch_bounds__(256) k_str_map(const SetSlot *probe, unsigned 
             const unsigned long long len = (unsigned long long)(offsets[row + 1] - offsets[row]);
             const unsigned long long h = murmur64(bytes + b, len);
             shard = (int)(h % (unsigned long long)nmaps);
-            ord = probe_lookup(probe, pmask, -1, h);
+            ord = set_ordinal(probe, pmask, -1, h);
             if (ord >= 0 && (str_len[ord] != len || !bytes_equal(pool + str_off[ord], bytes + b, len)))
                 ord = -1; // same hash, different string: not a member
         }
@@ -1843,15 +1741,8 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
     cudaStream_t st = call.st;
     StrInput in;
     B200_CHECK(stage_strings(call, offsets, bytes, masks, nrows, &in));
-    // room for the worst case of this call: every row a new key
+    B200_CHECK(set_reserve(s, st, nrows));
     {
-        uint64_t want = s->cap;
-        const uint64_t known = s->dirty ? 0 : (uint64_t)s->n_keys;
-        const uint64_t target = std::min<uint64_t>((known + (uint64_t)nrows) * 2, 1ull << 22);
-        while (want < target)
-            want <<= 1;
-        if (s->cap < want)
-            B200_CHECK(set_grow(s, st, want)); // one step (the cascade 4K -> 16K -> ... cost five allocations and rehashes)
         unsigned long long sc[2];
         B200_CUDA(cudaMemcpyAsync(sc, s->d_strctr, 16, cudaMemcpyDeviceToHost, st));
         B200_CUDA(cudaStreamSynchronize(st));
@@ -1872,21 +1763,13 @@ int b200_strset_update(b200_set *s, int slot, const int64_t *offsets, const uint
     const unsigned long long tag_base = (unsigned long long)s->seq << 40;
     s->seq++;
     s->max_call_rows = std::max<int64_t>(s->max_call_rows, nrows);
-    unsigned long long h[CTR_N];
-    int redo = 0;
-    for (int attempt = 0; nrows && attempt < 64; attempt++) {
-        k_str_insert<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->table, s->cap - 1, s->d_ctr, s->d_strctr, s->log, s->pool, s->slot_log, in.offsets, in.bytes,
-                                                                       in.masks, in.base, 0, nrows, tag_base, redo, kTagLowMask - 1);
-        B200_CUDA(cudaGetLastError());
-        B200_CHECK(read_ctr(s, st, h));
-        if (!h[CTR_OVERFLOW])
-            break;
-        unsigned long long zero = 0;
-        B200_CUDA(cudaMemcpyAsync(s->d_ctr + CTR_OVERFLOW, &zero, sizeof zero, cudaMemcpyHostToDevice, st));
-        B200_CHECK(set_grow(s, st));
-        redo = 2; // inserts are idempotent; the nulls of this call were already counted
-    }
     if (nrows) {
+        B200_CHECK(set_insert_pass(s, st, [&](int redo) -> int {
+            k_str_insert<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->table, s->cap - 1, s->d_ctr, s->d_strctr, s->log, s->pool, s->slot_log, in.offsets,
+                                                                           in.bytes, in.masks, in.base, 0, nrows, tag_base, redo, kTagLowMask - 1);
+            B200_CUDA(cudaGetLastError());
+            return B200_OK;
+        }));
         k_str_verify<<<nblocks((unsigned long long)nrows), 256, 0, st>>>(s->table, s->cap - 1, s->d_ctr, s->log, s->pool, s->slot_log, in.offsets, in.bytes, in.masks,
                                                                        in.base, nrows);
         B200_CUDA(cudaGetLastError());
