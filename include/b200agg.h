@@ -387,7 +387,19 @@ typedef enum {
     B200_EX_LT, B200_EX_LE, B200_EX_GT, B200_EX_GE, B200_EX_EQ, B200_EX_NE, /* -> bool */
     B200_EX_AND, B200_EX_OR, B200_EX_NOT,                                   /* on bools */
     B200_EX_CAST,   /* astype(b200_dtype arg) */
-    B200_EX_ORDINAL /* _ordinal_values(value, sets[arg]) -> int64 ordinal, -1 when absent (vaex/functions.py:2454-2463) */
+    B200_EX_ORDINAL, /* _ordinal_values(value, sets[arg]) -> int64 ordinal, -1 when absent (vaex/functions.py:2454-2463) */
+    /* the string calls of b200_str_eval (never in a b200_eval program: their results enter it as inputs) */
+    B200_EX_STR_EQUALS,     /* -> bool: row == pattern, False on a null row (src/superstring.hpp:200-234) */
+    B200_EX_STR_EQUALS2,    /* -> bool: row == the second column's row; null == null, null != any value (src/superstring.hpp:235-268) */
+    B200_EX_STR_STARTSWITH, /* -> bool (src/superstring.hpp:145-160) */
+    B200_EX_STR_ENDSWITH,   /* -> bool (src/superstring.hpp:130-144) */
+    B200_EX_STR_CONTAINS,   /* -> bool: the pattern occurs (src/strings.cpp:77-110, literal branch: string_view::find) */
+    B200_EX_STR_COUNT,      /* -> int64: non-overlapping occurrences, plen >= 1 (src/strings.cpp:31-75, literal branch) */
+    B200_EX_STR_FIND,       /* -> int64: byte offset of the first occurrence inside the code-point window [start, end), -1 when none */
+    B200_EX_STR_RFIND,      /*    or of the last one (src/superstring.hpp:161-197 with utf8_index_to_byte_offset and
+                                  utf8_slice_neg_index_to_byte_offset, :56-95) */
+    B200_EX_STR_LEN,        /* -> int64: UTF-8 code points by the lead-byte rule (src/string_utils.hpp:310-326) */
+    B200_EX_STR_BYTE_LENGTH /* -> int64 (src/superstring.hpp:1436-1438) */
 } b200_expr_opcode;
 /* I64_U64 / U64_I64: comparisons only, a signed integer (sign-extended) against a uint64, compared by exact value like numpy's
    mixed-sign comparison loops; the name gives the operands' order */
@@ -411,6 +423,18 @@ int b200_eval(b200_ctx *ctx, int slot, const b200_expr_op *prog, int nops, const
  * cols[c] in order; *count_out = rows kept (the call waits for it). */
 int b200_compact(b200_ctx *ctx, int slot, const uint8_t *keep, int ncols, const void *const *cols, const int32_t *dtypes, int64_t nrows, int memspace,
                  void *const *outs_device, int64_t *count_out);
+
+/* One string call of a device expression over nrows rows of an arrow string column: offsets = nrows + 1 int32 or int64 values
+ * (offset_isz 4 / 8, a sliced array's own offsets, used as they are), bytes = the byte the offset value 0 points at (the buffer the
+ * offsets index; only the bytes of the rows are read), nbytes = offsets[nrows] - offsets[0], nulls (may be NULL) = one byte a row,
+ * 1 = null.  Every row is read through its offsets, null or not; only B200_EX_STR_EQUALS / EQUALS2 look at nulls.  The second column
+ * (offsets2 ...) is read by B200_EX_STR_EQUALS2 only.  pattern = plen bytes (UTF-8); start / end: the code-point window of FIND /
+ * RFIND (end = INT64_MAX: to the end of the row).  A lead byte >= 0xF8 steps one byte in LEN, FIND and RFIND (the reference does not
+ * end on it); COUNT refuses an empty pattern (the reference never ends on it).  out_device: nrows bool or int64 (the opcode's result
+ * type).  Every pointer is device memory; the kernel is enqueued on the slot's stream (consume the result on the same slot). */
+int b200_str_eval(b200_ctx *ctx, int slot, int op, const void *offsets, int offset_isz, const uint8_t *bytes, const uint8_t *nulls, const void *offsets2,
+                  int offset2_isz, const uint8_t *bytes2, const uint8_t *nulls2, const uint8_t *pattern, int64_t plen, int64_t start, int64_t end,
+                  int64_t nrows, int64_t nbytes, void *out_device);
 
 /* ---- take: the row gather of df.join (vaex/join.py:286 right_dataset.take(lookup, masked=...), :214 left.take(lookup_left), :218-222
  * the inner join's matched rows) ----------------------------------------------------------------------------------------------

@@ -461,6 +461,10 @@ class Frame:
 
     def _agg(self, aggregators, binby=None, limits=None, shape=128, selection=None, edges=False, progress=None):
         """Run several aggregators in as few passes as possible (equal binners -> one fused pass); returns their results."""
+        # a binby expression that is not a column (e.g. str_len(name)) is binned as a device-evaluated column
+        f = self._with_columns([b for b in _binned_args(binby, shape, limits)[0] if isinstance(b, str)])
+        if f is not self:
+            return f._agg(aggregators, binby, limits, shape, selection, edges, progress)
         single = not isinstance(aggregators, (list, tuple))
         aggregators = [aggregators] if single else list(aggregators)
         specs = self._binner_specs(binby, limits, shape)

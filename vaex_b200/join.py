@@ -130,7 +130,9 @@ def take(index, columns, src_len, device):
 
 
 def _string_source(values):
-    """an arrow string / large_string array (or numpy object strings) -> (offsets, offset itemsize, bytes, mask or None)"""
+    """an arrow string / large_string array (or numpy object strings) -> (offsets, offset itemsize, bytes, first, mask or None).  `bytes`
+    are the rows' own bytes: offsets[0] .. offsets[n] of the buffer, which a slice of a long column shares with the whole column;
+    `first` = offsets[0] is the offset value of bytes[0], so the offsets index `bytes` shifted back by `first`."""
     import pyarrow as pa
     if isinstance(values, pa.ChunkedArray):
         values = values.combine_chunks()
@@ -140,41 +142,56 @@ def _string_source(values):
     n = len(values)
     validity, off_buf, data_buf = values.buffers()
     offsets = np.frombuffer(off_buf, dtype=np.int64 if isz == 8 else np.int32, count=n + 1, offset=values.offset * isz)
-    data = np.frombuffer(data_buf, dtype=np.uint8) if data_buf is not None and data_buf.size else np.zeros(1, np.uint8)
+    first, last = int(offsets[0]), int(offsets[-1])
+    data = np.frombuffer(data_buf, dtype=np.uint8)[first:last] if data_buf is not None and last > first else np.zeros(1, np.uint8)
     mask = None
     if values.null_count:
-        bits = np.unpackbits(np.frombuffer(validity, dtype=np.uint8), bitorder="little")[values.offset:values.offset + n]
+        lo = values.offset // 8  # unpack only the bytes of the rows in use: a chunk of a long column is a small slice of its bitmap
+        bits = np.unpackbits(np.frombuffer(validity, dtype=np.uint8)[lo:(values.offset + n + 7) // 8], bitorder="little")
+        bits = bits[values.offset - 8 * lo:values.offset - 8 * lo + n]
         mask = np.ascontiguousarray(1 - bits).astype(np.uint8)
-    return offsets, isz, data, mask
+    return offsets, isz, data, first, mask
 
 
-def take_strings(index, values):
+def take_strings(index, values, thread_index=None):
     """b200_take_strings: the arrow string column `values` gathered by `index` -> (pyarrow large_string array with nulls where a row is
-    missing, whether a row was missing)"""
+    missing, whether a row was missing).  Only the bytes of `values`' own rows are copied to the device.  With `thread_index` the
+    gather runs on that worker's slot, after the work already queued there (filter compaction gathers by the kept rows it computed
+    on that slot), and waits for that slot only; without it, on slot 0 after every slot and torch's stream."""
+    import contextlib
+
     import pyarrow as pa
     torch = _torch()
     ctx = _lib.context()
-    ctx.sync()
-    idx = _staged_index(index)
-    n = len(idx)
-    offsets, isz, data, mask = _string_source(values)
-    src_len = len(offsets) - 1
-    d_off, d_data = _staged(offsets), _staged(data)
-    d_mask = None if mask is None else _staged(mask)
-    out_off = torch.empty(n + 1, dtype=torch.int64, device=idx.device)
-    valid = torch.empty(max(n, 1), dtype=torch.uint8, device=idx.device)
-    size, missing = C.c_int64(0), C.c_int32(0)
-    torch.cuda.synchronize(idx.device)  # the staging copies run on torch's stream, the gather on a slot's
-    args = (ctx._h, 0, idx.data_ptr(), idx.element_size(), n, d_off.data_ptr(), isz, d_data.data_ptr(), None if d_mask is None else d_mask.data_ptr(),
-            src_len, out_off.data_ptr())
-    _lib.check(_lib.lib().b200_take_strings(*args, None, valid.data_ptr(), 0, C.byref(size), C.byref(missing)))
-    out_bytes = torch.empty(max(size.value, 1), dtype=torch.uint8, device=idx.device)
-    if size.value:
-        _lib.check(_lib.lib().b200_take_strings(*args, out_bytes.data_ptr(), valid.data_ptr(), size.value, C.byref(size), C.byref(missing)))
-    valid = valid[:n].cpu().numpy()
+    if thread_index is None:
+        ctx.sync()
+        slot, stream = 0, contextlib.nullcontext()
+    else:
+        slot = ctx.slot(thread_index)
+        stream = torch.cuda.stream(torch.cuda.ExternalStream(ctx.stream(slot), device=f"cuda:{ctx.device}"))
+    with stream:  # a slot's stream: the copies and temporaries are ordered with the gather, torch's cache reuses them after it
+        idx = _staged_index(index)
+        n = len(idx)
+        offsets, isz, data, first, mask = _string_source(values)
+        src_len = len(offsets) - 1
+        d_off, d_data = _staged(offsets), _staged(data)
+        d_mask = None if mask is None else _staged(mask)
+        out_off = torch.empty(n + 1, dtype=torch.int64, device=idx.device)
+        valid = torch.empty(max(n, 1), dtype=torch.uint8, device=idx.device)
+        size, missing = C.c_int64(0), C.c_int32(0)
+        if thread_index is None:
+            torch.cuda.synchronize(idx.device)  # the staging copies run on torch's stream, the gather on a slot's
+        # the device pointer the offsets index: the staged bytes start at offset value `first`
+        args = (ctx._h, slot, idx.data_ptr(), idx.element_size(), n, d_off.data_ptr(), isz, d_data.data_ptr() - first,
+                None if d_mask is None else d_mask.data_ptr(), src_len, out_off.data_ptr())
+        _lib.check(_lib.lib().b200_take_strings(*args, None, valid.data_ptr(), 0, C.byref(size), C.byref(missing)))
+        out_bytes = torch.empty(max(size.value, 1), dtype=torch.uint8, device=idx.device)
+        if size.value:
+            _lib.check(_lib.lib().b200_take_strings(*args, out_bytes.data_ptr(), valid.data_ptr(), size.value, C.byref(size), C.byref(missing)))
+        valid = valid[:n].cpu().numpy()
+        off_host, bytes_host = out_off.cpu().numpy(), out_bytes[:size.value].cpu().numpy()
     bitmap = pa.py_buffer(np.packbits(valid.astype(bool), bitorder="little")) if missing.value else None
-    arr = pa.LargeStringArray.from_buffers(n, pa.py_buffer(out_off.cpu().numpy()), pa.py_buffer(out_bytes[:size.value].cpu().numpy()), bitmap,
-                                           int(n - valid.sum()) if missing.value else 0)
+    arr = pa.LargeStringArray.from_buffers(n, pa.py_buffer(off_host), pa.py_buffer(bytes_host), bitmap, int(n - valid.sum()) if missing.value else 0)
     return arr, bool(missing.value)
 
 
