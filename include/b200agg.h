@@ -436,6 +436,19 @@ int b200_str_eval(b200_ctx *ctx, int slot, int op, const void *offsets, int offs
                   int offset2_isz, const uint8_t *bytes2, const uint8_t *nulls2, const uint8_t *pattern, int64_t plen, int64_t start, int64_t end,
                   int64_t nrows, int64_t nbytes, void *out_device);
 
+/* The point-in-polygon test of a lasso selection (vaex/selections.py:172-201 over vaexfast.pnpoly, src/vaexfast.cpp:1856-1874):
+ * out_device[r] = 1 when row r's float64 (x, y) lies inside the polygon by the crossing-number rule, 0 otherwise, and 0 without a
+ * test when (x - meanx)^2 + (y - meany)^2 < radius^2 fails.  meanx, meany and radius are the reference's, computed on the host.
+ * edges = 4 doubles an edge, (x_i, y_i, x_j, y_j) for j = i - 1.  nbands = 0: every row tests the nedges edges (the reference's
+ * loop).  nbands > 0: band_start holds nbands + 1 offsets into edges; a row with band_lo <= y < band_hi tests only the edges of
+ * band clamp((int)((y - band_lo) * band_scale), 0, nbands - 1), other rows none, so every edge with min(y_i, y_j) <= y < max(y_i,
+ * y_j) for a row that maps to a band must be listed in that band.  The arithmetic is the reference's, one rounding an operation and
+ * no FMA, so both forms give its answer bit for bit.  Every pointer is device memory; the kernel is enqueued on the slot's stream
+ * (consume the result on the same slot).  Bound: HBM reads of x and y for small polygons, fp64 compares of the band's edges for
+ * large ones (DESIGN.md §4). */
+int b200_lasso(b200_ctx *ctx, int slot, const double *x, const double *y, int64_t nrows, const double *edges, int64_t nedges, const int32_t *band_start,
+               int32_t nbands, double band_lo, double band_hi, double band_scale, double meanx, double meany, double radius, uint8_t *out_device);
+
 /* ---- take: the row gather of df.join (vaex/join.py:286 right_dataset.take(lookup, masked=...), :214 left.take(lookup_left), :218-222
  * the inner join's matched rows) ----------------------------------------------------------------------------------------------
  * index: n rows of int8/16/32/64 (index_isz 1/2/4/8), the row of the source each output row takes; < 0 = missing (value 0, validity

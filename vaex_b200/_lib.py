@@ -16,7 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # VAEX_B200_LIB: load this build of the library instead of the in-tree one (A/B timing of kernel variants on one box)
 LIB_PATH = os.environ.get("VAEX_B200_LIB") or os.path.join(_HERE, "libb200agg.so")
 CSRC = os.path.join(_HERE, "csrc")
-SOURCES = ["api.cu", "binby.cu", "expr.cu", "fast.cu", "first.cu", "hashset.cu", "list.cu", "minmax.cu", "mutinfo.cu", "nunique.cu", "percentile.cu",
+SOURCES = ["api.cu", "binby.cu", "expr.cu", "fast.cu", "first.cu", "hashset.cu", "lasso.cu", "list.cu", "minmax.cu", "mutinfo.cu", "nunique.cu", "percentile.cu",
            "ringcount.cu", "sort.cu", "statistic.cu", "strexpr.cu", "take.cu", "tilesort.cu"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
@@ -136,6 +136,7 @@ def lib():
             "b200_bin": (i32, [vp, i32, P(Binner), i32, P(AggInput), i32, i64, i64, i32, u32]),
             "b200_eval": (i32, [vp, i32, P(ExprOp), i32, P(ExprInput), i32, P(vp), i32, i64, i32, i32, vp]),
             "b200_str_eval": (i32, [vp, i32, i32, vp, i32, vp, vp, vp, i32, vp, vp, vp, i64, i64, i64, i64, i64, vp]),
+            "b200_lasso": (i32, [vp, i32, vp, vp, i64, vp, i64, vp, i32, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, vp]),
             "b200_compact": (i32, [vp, i32, vp, i32, P(vp), P(i32), i64, i32, P(vp), P(i64)]),
             "b200_take": (i32, [vp, i32, vp, i32, i64, i32, P(vp), P(i32), P(vp), i64, P(vp), P(vp), P(i32)]),
             "b200_take_strings": (i32, [vp, i32, vp, i32, i64, vp, i32, vp, vp, i64, vp, vp, vp, i64, P(i64), P(i32)]),

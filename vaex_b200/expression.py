@@ -531,6 +531,11 @@ class DeviceExpression:
         return outs
 
     def chunk(self, thread_index, i1, i2):
+        return self.run(thread_index, i1, i2, [self._columns[name][i1:i2] for name in self.program.inputs])
+
+    def run(self, thread_index, i1, i2, parts):
+        """the program over rows [i1, i2) with `parts` as the blocks of its column inputs, in program.inputs order (a selection feeds
+        the masks it computes this way, vaex_b200/selections.py)"""
         n = int(i2 - i1)
         raw = self._buffer(thread_index, n)
         out = DeviceArray(raw.data_ptr(), n, self.dtype, keep=raw)
@@ -539,8 +544,7 @@ class DeviceExpression:
         nin = len(self.program.inputs) + len(self.program.strcalls)
         inputs = (_lib.ExprInput * max(nin, 1))()
         keep = []
-        for k, name in enumerate(self.program.inputs):
-            part = self._columns[name][i1:i2]
+        for k, part in enumerate(parts):
             if isinstance(part, np.ndarray) and not part.dtype.isnative:
                 part = part.astype(part.dtype.newbyteorder("="))
             c = _lib.column(part)

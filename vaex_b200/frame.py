@@ -7,13 +7,14 @@ Columns are plain arrays: numpy (host; streamed in chunks) or device arrays (tor
 Expressions are column NAMES only — the expression system is upstream of the path and out of scope.
 """
 import ast
+import collections
 import re
 
 import numpy as np
 
 from . import _lib
 from . import agg as _agg
-from . import execution, taskpart
+from . import execution, selections, taskpart
 from . import hash as _hash
 from .groupby import Binner, BinnerBase, BinnerInteger, BinnerTime  # noqa: F401  (vaex.groupby's binners, for Frame.groupby)
 
@@ -33,6 +34,9 @@ class Frame:
         n = {len(v) for v in self.columns.values()}
         assert len(n) <= 1, "all columns must have equal length"
         self.length = n.pop() if n else 0
+        # named selections (vaex/dataframe.py:205-206): per name a history of selection objects and the index of the current one
+        self.selection_histories = collections.defaultdict(list)
+        self.selection_history_indices = collections.defaultdict(lambda: -1)
         if filter is not None:
             self._filter = self.expression(filter)
             if self._filter.dtype != np.bool_:
@@ -46,7 +50,12 @@ class Frame:
         true, its filter; the filter is compiled again because a compiled expression is bound to its frame's column dict"""
         if filter is None and not drop_filter:
             filter = self._filter_expression
-        return Frame(columns, executor=self.executor, categories=self.categories, filter=filter, variables=self.variables)
+        f = Frame(columns, executor=self.executor, categories=self.categories, filter=filter, variables=self.variables)
+        # a copy of the selection histories, as vaex's copy() takes (vaex/dataframe.py:3293-3298)
+        for name, history in self.selection_histories.items():
+            f.selection_histories[name] = list(history)
+        f.selection_history_indices.update(self.selection_history_indices)
+        return f
 
     def _with_columns(self, names):
         """this frame when every name is one of its columns, else a derived frame in which each missing name is a device-evaluated
@@ -59,19 +68,124 @@ class Frame:
             f.columns[e] = f.expression(e)
         return f
 
-    def _selection(self, selection):
+    def _selection(self, selection, memo=None):
         """a selection argument -> None for None / False, a boolean device expression for a string, a mask array as it is, and a
-        list of selections element by element"""
+        list of selections element by element.  True means the selection named "default"; a string that names selections of this
+        frame (and no column) is resolved through them (selections.resolve_text), every name to one object within the call."""
         if isinstance(selection, (list, tuple)):
-            return [self._selection(one) for one in selection]
+            memo = {} if memo is None else memo
+            return [self._selection(one, memo) for one in selection]
         if selection is None or selection is False:
             return None
+        if selection is True:
+            return _boolean_selection(selections.resolve_text(self, "default", memo))
         if isinstance(selection, str):
-            mask = self.expression(selection)
-            if mask.dtype != np.bool_:
-                raise ValueError("a selection must be a boolean expression")
-            return mask
+            try:
+                mask = self.expression(selection)
+            except KeyError:
+                if not selections.names_selection(self, selection):
+                    raise
+                mask = selections.resolve_text(self, selection, memo)
+            return _boolean_selection(mask)
         return selection
+
+    # ---- named selections (vaex/dataframe.py:5000-5303), evaluated on the device (vaex_b200/selections.py) ------------------------
+    def get_selection(self, name="default"):
+        """the current selection object of `name`, None when there is none"""
+        name = "default" if name is True else name
+        history = self.selection_histories[name]
+        index = self.selection_history_indices[name]
+        return None if index == -1 else history[index]
+
+    def has_selection(self, name="default"):
+        return self.get_selection(name) is not None
+
+    def _has_history(self, name):
+        """whether `name` is a selection of this frame that selects something, without adding an empty history for it"""
+        return bool(self.selection_histories.get(name)) and self.get_selection(name) is not None
+
+    def selection_can_undo(self, name="default"):
+        return self.selection_history_indices[name] > -1
+
+    def selection_can_redo(self, name="default"):
+        return (self.selection_history_indices[name] + 1) < len(self.selection_histories[name])
+
+    def selection_undo(self, name="default"):
+        if not self.selection_can_undo(name=name):
+            raise ValueError(f"selection {name!r} has nothing to undo")
+        self.selection_history_indices[name] -= 1
+
+    def selection_redo(self, name="default"):
+        if not self.selection_can_redo(name=name):
+            raise ValueError(f"selection {name!r} has nothing to redo")
+        self.selection_history_indices[name] += 1
+
+    def _push_selection(self, create, name, check=True):
+        """DataFrame._selection (vaex/dataframe.py:5285-5299): the new entry goes after the current one and the redo tail is clipped.
+        The current entry is the reference's: with the index at -1 and a non-empty history that is the LAST entry.  `check`
+        resolves the new entry first, so a selection that cannot be evaluated is refused before it is recorded."""
+        history = self.selection_histories[name]
+        current = history[self.selection_history_indices[name]] if history else None
+        selection = create(current)
+        if check and selection is not None:
+            _boolean_selection(selections.resolve(self, selection, stack=(name,)))
+        history.append(selection)
+        self.selection_history_indices[name] += 1
+        del history[self.selection_history_indices[name]:-1]
+
+    def select(self, boolean_expression, mode="replace", name="default"):
+        """df.select (vaex/dataframe.py:5041-5059): select by a boolean expression, combined with the current selection of `name` by
+        `mode` (replace / and / or / xor / subtract).  None clears the selection (and records nothing when there is none)."""
+        if boolean_expression is not None:
+            boolean_expression = str(boolean_expression)
+        if boolean_expression is None and not self.has_selection(name=name):
+            return
+        self._push_selection(lambda current: selections.SelectionExpression(boolean_expression, current, mode) if boolean_expression else None, name)
+
+    def select_nothing(self, name="default"):
+        self.select(None, name=name)
+
+    def select_rectangle(self, x, y, limits, mode="replace", name="default"):
+        self.select_box([x, y], limits, mode=mode, name=name)
+
+    def select_box(self, spaces, limits, mode="replace", name="default"):
+        """df.select_box (vaex/dataframe.py:5156-5173): the reference's text, each limit written with %f"""
+        self.select(selections.box_text(spaces, limits), mode=mode, name=name)
+
+    def select_circle(self, x, y, xc, yc, r, mode="replace", name="default", inclusive=True):
+        """df.select_circle (vaex/dataframe.py:5175-5199); the squares are written as products (selections.Text)"""
+        self.select(selections.circle_text(x, y, xc, yc, r, inclusive).device, mode=mode, name=name)
+
+    def select_ellipse(self, x, y, xc, yc, width, height, angle=0, mode="replace", name="default", radians=False, inclusive=True):
+        """df.select_ellipse (vaex/dataframe.py:5201-5242); the squares are written as products (selections.Text)"""
+        text = selections.ellipse_text(x, y, xc, yc, width, height, angle, radians=radians, inclusive=inclusive)
+        self.select(text.device, mode=mode, name=name)
+
+    def select_lasso(self, expression_x, expression_y, xsequence, ysequence, mode="replace", name="default"):
+        """df.select_lasso (vaex/dataframe.py:5244-5259): the rows whose (x, y) lie inside the polygon, tested on the device
+        (b200_lasso); a row with a masked x or y is never selected"""
+        self._push_selection(lambda current: selections.SelectionLasso(expression_x, expression_y, xsequence, ysequence, current, mode), name)
+
+    def select_inverse(self, name="default"):
+        """df.select_inverse (vaex/dataframe.py:5261-5271); without a selection to invert it raises and records nothing"""
+        history = self.selection_histories[name]
+        if (history[self.selection_history_indices[name]] if history else None) is None:
+            raise ValueError(f"select_inverse: there is no selection {name!r} to invert")
+        self._push_selection(selections.SelectionInvert, name)
+
+    def select_non_missing(self, drop_nan=True, drop_masked=True, column_names=None, mode="replace", name="default"):
+        """df.select_non_missing (vaex/dataframe.py:5061-5077): the rows with no NaN (drop_nan) and no missing value (drop_masked:
+        masked, arrow null, None) in any of `column_names`, by default every real column"""
+        from . import expression as _expr
+        column_names = column_names or [k for k, v in self.columns.items() if not isinstance(v, _expr.DeviceExpression)]
+        self._push_selection(lambda current: selections.SelectionDropNa(drop_nan, drop_masked, [str(k) for k in column_names], current, mode), name)
+
+    def set_selection(self, selection, name="default"):
+        self._push_selection(lambda current: selection, name)
+
+    def selected_length(self, selection="default"):
+        """the number of rows the selection selects (vaex/dataframe.py:7122-7124)"""
+        return int(np.asarray(self.count(selection=selection)).item())
 
     # ---- expressions: virtual columns, filters, selections — evaluated on the device (csrc/expr.cu) ----------------------------
     def expression(self, text):
@@ -836,6 +950,13 @@ class GroupBy:
             out[label] = _take_cells(g, flat) if _is_arrow(g) else g[center][keep]
         out["count"] = counts[keep]
         return out
+
+
+def _boolean_selection(mask):
+    """a resolved selection argument, checked to be boolean"""
+    if mask.dtype != np.bool_:
+        raise ValueError("a selection must be a boolean expression")
+    return mask
 
 
 def _issequence(x):
