@@ -8,7 +8,8 @@
 // crowded distribution spreads evenly over them), else a contiguous range of the index:
 //
 //   K1 k_ring_partition  every WARP is autonomous.  The keys of the NEXT 256-row group are loaded into registers (128-bit,
-//                        evict-first loads) while the current group is placed.
+//                        evict-first loads) while the current group is placed, and the group after that is bulk-prefetched
+//                        into L2 (one cp.async.bulk.prefetch per key column).
 //                        Per row: the bit-exact fp64 bin index, the part (outer cell mod parts, or idx / tile_cells by one
 //                        IMAD.HI), ONE shared-memory atomic
 //                        on the (warp, part) counter whose return value is the row's slot in that part's RING (96 entries), and
@@ -351,6 +352,17 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
             for (int d = 0; d < ND; d++)
                 ldcs4<T>(p.x[d], r0 + q * 128, dst[q][d]);
     };
+    // the warp's group two turns ahead goes into L2 with one bulk prefetch per key column (lane d: column d).  The register
+    // loads reach only one group ahead; without this the warp has no load in flight once they land, and HBM sees too few
+    // requests (3.72 -> 3.55 ms per 1e9 rows on an H100 80GB HBM3 at 700 W; three turns ahead gained nothing).  Columns are
+    // 16-byte aligned and batches start on a 256-row boundary, so every group is 16-byte aligned.
+    constexpr long long kPrefetch = 2;
+    auto prefetch = [&](long long g) {
+        if (lane < ND && g < ngroups) {
+            const T *src = static_cast<const T *>(p.x[lane]) + p.row0 + g * kGroupRows;
+            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"((unsigned)(kGroupRows * sizeof(T))) : "memory");
+        }
+    };
     auto place = [&](const T (&c)[2][ND][4]) {
         unsigned idx[8], slots[8];
         const unsigned worst = group_rows_regs<T, ND, RING, RSTRIDE, CLAMPED, PPL, ILV>(p, c, cnt, ring, idx, slots);
@@ -366,12 +378,14 @@ __global__ void __launch_bounds__(WARPS * 32, 2) k_ring_partition(const __grid_c
         if (g < ngroups)
             load(g, ca);
         while (g < ngroups) {
+            prefetch(g + kPrefetch * wtotal);
             if (g + wtotal < ngroups)
                 load(g + wtotal, cb);
             place(ca);
             g += wtotal;
             if (g >= ngroups)
                 break;
+            prefetch(g + kPrefetch * wtotal);
             if (g + wtotal < ngroups)
                 load(g + wtotal, ca);
             place(cb);
