@@ -67,7 +67,8 @@ def _staged(x):
     and unsigned integers travel as signed integers of their width)"""
     torch = _torch()
     if _lib.is_device(x):
-        return _device_tensor(x)
+        # torch has no datetime64 / timedelta64: a device datetime column travels as its int64 ticks, as a host one does
+        return _device_tensor(_lib.int64_view(x) if _lib.dtype_of(x).kind in "mM" else x)
     a = np.ascontiguousarray(x)
     if a.dtype.kind in "mMu" and a.dtype.itemsize > 1:
         a = a.view(f"i{a.dtype.itemsize}")
